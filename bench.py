@@ -1,11 +1,16 @@
 #!/usr/bin/env python
-"""bench.py — compaction throughput of the B200 engine on BASELINE.json's metric.
+"""bench.py — compaction throughput of the H100 engine on BASELINE.json's metric.
 
   python bench.py --gpus N --steps K --warmup W            (N>1: launched by torchrun, one rank per GPU)
   python bench.py --impl reference --gpus N --steps K --warmup W
+  python bench.py --gpus 1 --steps K --warmup W --dump-outputs DIR
+
+Every timed loop below runs --steps steps after --warmup untimed ones (configs[4]: at least one warm-up).
 
 A "step" is one whole compaction job over the workload (SURVEY.md 8d / BASELINE.md §3 config 2:
-8-way major compaction, 100 M entries, 32-B DocKey + 256-B value, kNoCompression SSTs). With N>1
+8-way major compaction, 32-B DocKey + 256-B value, kNoCompression SSTs; 40 M entries per GPU, sized so that
+the single-job end-to-end arm — inputs, intermediates and output resident at once — stays well inside the 80 GB of
+an H100). With N>1
 every rank compacts its own tablet of that shape (tablets are independent: no data-path
 collective, weak scaling).
 
@@ -23,8 +28,7 @@ entries, as rocksdb.raw.key.size + rocksdb.raw.value.size count them).
             e2e.range_files = the same with one SST per range (ybgpu_compact_files);
             e2e.single_job = one job, H2D / run / D2H back to back. e2e.pcie_ceiling_gbs = concurrent
             bidirectional copies of the same pinned buffers, measured in this run.
-  roofline  dominant kernel, algorithmic bytes / its CUDA-event time (see DESIGN.md); roofline.traffic is
-            read from the committed ncu capture under profiles/ (traffic_source says which), not measured here.
+  roofline  dominant kernel, algorithmic bytes / its CUDA-event time (see DESIGN.md).
   configs   BASELINE configs[2] (64 tablets x 4-way x 10 M: 8 tablets per GPU) and configs[3] (MVCC-heavy, the
             largest size resident on one GPU) as sub-results with their own pipeline roofline.
   cpu_baseline  the oracle (CPU restatement of the reference loop) on a bounded sample, 1 thread like the
@@ -32,6 +36,17 @@ entries, as rocksdb.raw.key.size + rocksdb.raw.value.size count them).
             threads running independent one-thread compactions.
   parity_check  the GPU engine compacts the cpu_baseline sample files in this run: counters, KV hash and the
             SHA-256 of both output files must equal the oracle's.
+  gpu       device name and power limit the numbers were measured at.
+
+--dump-outputs DIR: after the timed steps, what the last timed job of the headline (HBM-resident) arm returned to its
+caller, as .npy files small enough to compare two builds output for output (inputs are seeded: identical from run to
+run with the same arguments):
+  stats.npy              float64 (14, 2): the job's counters (JobStats fields up to largest_seqno), each as
+                         (high 32 bits, low 32 bits)
+  output_sha256.npy      float64 (2, 8): SHA-256 of the output data file and of the metadata file, as 32-bit words
+  output_data_sample.npy float32 (windows, 1024): bytes of the output data file at seeded window offsets
+  output_data_offsets.npy float64: those offsets
+  output_meta_sample.npy, output_meta_offsets.npy: the same for the metadata file (the whole file when it is small)
 """
 import argparse
 import ctypes
@@ -46,10 +61,11 @@ import time
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
-DEFAULT_ROWS = 100_000_000       # config 2: 100 M entries
+DEFAULT_ROWS = 40_000_000        # config 2 shape, 40 M entries (12.4 GB of raw key + value bytes) per GPU
 VALUE_LEN = 256
 NUM_FILES = 8
-WORKLOAD = "8-way major compaction, 100M keys, 32-B DocKey / 256-B value, 1 GPU"
+WORKLOAD = "8-way major compaction, 40M keys, 32-B DocKey / 256-B value, 1 GPU"
+H100_HBM_GBS = 3350.0            # NVIDIA H100 SXM data sheet (700 W): the peak when MEASURED_PEAKS.json is absent
 
 
 def parse_args():
@@ -69,14 +85,16 @@ def parse_args():
     ap.add_argument("--no-extra-configs", action="store_true", help="skip the BASELINE configs[2] / configs[3] sub-results")
     ap.add_argument("--c3-tablets", type=int, default=8, help="configs[2]: tablets per GPU (64 tablets / 8 GPUs)")
     ap.add_argument("--c3-rows", type=int, default=10_000_000, help="configs[2]: entries per tablet")
-    ap.add_argument("--c4-rows", type=int, default=200_000_000,
+    ap.add_argument("--c4-rows", type=int, default=80_000_000,
                     help="configs[3] (MVCC-heavy, 20 versions/key): entries resident on one GPU (the full 1 G entries = 310 GB do not fit HBM)")
-    ap.add_argument("--c5-rows-per-gpu", type=int, default=40_000_000,
+    ap.add_argument("--c5-rows-per-gpu", type=int, default=16_000_000,
                     help="configs[4] (one oversized tablet, 32-way, key-range sharded over the GPUs with NCCL): entries per GPU")
     ap.add_argument("--c5-timeout", type=float, default=240.0, help="configs[4]: give up (and still print the line) after this many seconds")
     ap.add_argument("--workload", default="config2", choices=["config2", "mvcc"],
                     help="config2 = BASELINE configs[1] (the bench line); mvcc = configs[3] shape (20 versions/key, "
-                         "history cutoff drops 90 %), scaled to --rows entries, for profiles/ only")
+                         "history cutoff drops 90 %%), scaled to --rows entries, for profiles/ only")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step of the headline arm computed to DIR/*.npy (see the module docstring)")
     return ap.parse_args()
 
 
@@ -87,11 +105,11 @@ def measured_peaks():
             return json.load(open(p)), "measured"
         except Exception:
             pass
-    return {"hbm_gbs": 6650.0}, "fallback"
+    return {"hbm_gbs": H100_HBM_GBS}, "H100 SXM data sheet"
 
 
 class ClockSampler:
-    """nvidia-smi clocks + throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks, power limit and throttle reasons during the timed region."""
 
     def __init__(self, index):
         self.index = index
@@ -101,7 +119,7 @@ class ClockSampler:
     def start(self):
         q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
              "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
-             "clocks_event_reasons.sw_power_cap")
+             "clocks_event_reasons.sw_power_cap,power.limit")
         try:
             self.proc = subprocess.Popen(["nvidia-smi", "-i", str(self.index), "--query-gpu=" + q,
                                           "--format=csv,noheader,nounits", "-lms", "200"],
@@ -114,12 +132,12 @@ class ClockSampler:
     def _read(self):
         for line in self.proc.stdout:
             parts = [x.strip() for x in line.split(",")]
-            if len(parts) >= 7:
+            if len(parts) >= 8:
                 self.samples.append(parts)
 
     def stop(self):
         if not self.proc:
-            return {"sm_mhz": None, "sm_max_mhz": None, "reasons": ["nvidia-smi unavailable"]}
+            return {"sm_mhz": None, "sm_max_mhz": None, "power_limit_w": None, "reasons": ["nvidia-smi unavailable"]}
         self.proc.terminate()
         try:
             self.proc.wait(timeout=2)
@@ -127,12 +145,14 @@ class ClockSampler:
             self.proc.kill()
         sm = sorted(int(float(s[0])) for s in self.samples if s[0].replace(".", "").isdigit())
         mx = [int(float(s[1])) for s in self.samples if s[1].replace(".", "").isdigit()]
+        pl = [float(s[7]) for s in self.samples if s[7].replace(".", "").isdigit()]
         reasons = set()
         for s in self.samples:
             for name, v in zip(("hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"), s[3:7]):
                 if v.lower().startswith("active"):
                     reasons.add(name)
         return {"sm_mhz": sm[len(sm) // 2] if sm else None, "sm_max_mhz": max(mx) if mx else None,
+                "power_limit_w": max(pl) if pl else None,
                 "reasons": sorted(reasons), "samples": len(self.samples)}
 
 
@@ -315,9 +335,12 @@ def emit_json_line(line):
         sys.stdout.flush()
 
 
-def resident_arm(pkg, torch, ssts, handles, local_rank, stream_ptr, job_kw, verify, steps, warmup, barrier, world, dist, sample_clocks=False):
+def resident_arm(pkg, torch, ssts, handles, local_rank, stream_ptr, job_kw, verify, steps, warmup, barrier, world, dist, sample_clocks=False,
+                 keep_last=False):
     """`steps` whole jobs with the input files resident in HBM, timed between barriers (CUDA events + wall clock,
-    max over ranks). Returns (total seconds, per-step stats, clocks, host ms per phase)."""
+    max over ranks). Returns (total seconds, per-step stats, clocks, host ms per phase, last job). With keep_last the
+    last timed job is not closed (its close is then outside the timing) and is returned for dump_outputs; otherwise
+    the last job is None."""
     dev_files = []
     for s in ssts:
         v = s.data_view()
@@ -326,7 +349,9 @@ def resident_arm(pkg, torch, ssts, handles, local_rank, stream_ptr, job_kw, veri
         dev_files.append(t)
     host_ms = {"create": 0.0, "add_inputs": 0.0, "run": 0.0, "close": 0.0}
 
-    def step():
+    last = [None]
+
+    def step(keep=False):
         t0 = time.perf_counter()
         job = pkg.GpuCompactionJob(device=local_rank, verify_checksums=bool(verify), cuda_stream=stream_ptr, **job_kw)
         t1 = time.perf_counter()
@@ -336,7 +361,10 @@ def resident_arm(pkg, torch, ssts, handles, local_rank, stream_ptr, job_kw, veri
         st = job.run()
         t3 = time.perf_counter()
         d = st.as_dict()
-        job.close()
+        if keep:
+            last[0] = job
+        else:
+            job.close()
         t4 = time.perf_counter()
         for k, v in zip(("create", "add_inputs", "run", "close"), (t1 - t0, t2 - t1, t3 - t2, t4 - t3)):
             host_ms[k] += v * 1e3
@@ -353,7 +381,7 @@ def resident_arm(pkg, torch, ssts, handles, local_rank, stream_ptr, job_kw, veri
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     t0 = time.perf_counter()
     e0.record()
-    stats = [step() for _ in range(steps)]
+    stats = [step(keep_last and i == steps - 1) for i in range(steps)]
     e1.record()
     barrier()
     wall = time.perf_counter() - t0
@@ -362,8 +390,40 @@ def resident_arm(pkg, torch, ssts, handles, local_rank, stream_ptr, job_kw, veri
     tt = torch.tensor([step_s], dtype=torch.float64, device="cuda")
     if world > 1:
         dist.all_reduce(tt, op=dist.ReduceOp.MAX)
-    del dev_files
-    return float(tt.item()), stats, clock_info, {k: round(v / steps, 3) for k, v in host_ms.items()}
+    if last[0] is None:
+        del dev_files
+    else:
+        last[0].dev_files = dev_files          # the job reads its inputs from these buffers until it is closed
+    return float(tt.item()), stats, clock_info, {k: round(v / steps, 3) for k, v in host_ms.items()}, last[0]
+
+
+def dump_outputs(job, out_dir, window=1024, data_windows=4096, meta_windows=2048):
+    """Writes what `job` returned to its caller (counters, output data file, metadata file) to out_dir/*.npy: the
+    counters exactly, both files as SHA-256 and as seeded samples of 1 KB windows. At most
+    (data_windows + meta_windows) * window * 4 bytes of samples (24 MB)."""
+    import hashlib
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    st = job.stats()
+    names = [n for n, _ in st._fields_[:14]]
+    assert names[-1] == "largest_seqno"
+    stats = np.array([[getattr(st, n) >> 32, getattr(st, n) & 0xffffffff] for n in names], dtype=np.float64)
+    np.save(os.path.join(out_dir, "stats.npy"), stats)
+    data, meta = job.fetch_output()
+    sha = [np.frombuffer(hashlib.sha256(memoryview(f)).digest(), dtype=">u4").astype(np.float64) for f in (data, meta)]
+    np.save(os.path.join(out_dir, "output_sha256.npy"), np.stack(sha))
+    rng = np.random.default_rng(20241015)
+    for name, f, n in (("data", data, data_windows), ("meta", meta, meta_windows)):
+        if f.size <= n * window:
+            offs = np.arange(0, f.size, window, dtype=np.int64)
+        else:
+            offs = np.sort(rng.integers(0, f.size - window + 1, size=n, dtype=np.int64))
+        sample = np.zeros((offs.size, window), np.float32)
+        for i, o_ in enumerate(offs):
+            chunk = f[o_:o_ + window]
+            sample[i, :chunk.size] = chunk
+        np.save(os.path.join(out_dir, "output_%s_sample.npy" % name), sample)
+        np.save(os.path.join(out_dir, "output_%s_offsets.npy" % name), offs.astype(np.float64))
 
 
 def pipeline_roofline(stats, in_bytes, hbm_peak, steps):
@@ -391,6 +451,7 @@ def main():
     if not torch.cuda.is_available() or pkg.device_count() < 1:
         raise SystemExit("bench.py needs a CUDA device: the compaction engine has no CPU fallback")
     torch.cuda.set_device(local_rank)
+    props = torch.cuda.get_device_properties(local_rank)
     # Host placement first: every buffer this rank allocates below (generated input files, pinned output arenas) and
     # every thread it starts must sit on the NUMA node of its GPU, or the e2e arm pays the inter-socket link
     # (profiles/h2d_d2h_ceiling.py measures the difference).
@@ -410,7 +471,7 @@ def main():
         torch.cuda.synchronize()
 
     peaks, peak_kind = measured_peaks()
-    hbm_peak = float(peaks.get("hbm_gbs", 6650.0))
+    hbm_peak = float(peaks.get("hbm_gbs", H100_HBM_GBS))
 
     # ---- inputs: this rank's tablet (distinct key range per rank) ----
     versions = 20 if args.workload == "mvcc" else 1
@@ -435,10 +496,15 @@ def main():
 
     # ---- HBM-resident arm: checksum verification ON like the reference (verify_checksums_in_compaction = true,
     # rocksdb/util/options.cc:135, db/version_set.cc:3791-3792); the no-verify figure rides along ----
-    total_s, stats, clock_info, host_ms = resident_arm(pkg, torch, ssts, handles, local_rank, stream_ptr, job_kw, args.verify,
-                                                       args.steps, args.warmup, barrier, world, dist, sample_clocks=True)
-    nv_steps = max(1, min(args.steps, 5))
-    nv_s, nv_stats, _, _ = resident_arm(pkg, torch, ssts, handles, local_rank, stream_ptr, job_kw, 0, nv_steps, 1, barrier, world, dist)
+    total_s, stats, clock_info, host_ms, last_job = resident_arm(pkg, torch, ssts, handles, local_rank, stream_ptr, job_kw, args.verify,
+                                                                 args.steps, args.warmup, barrier, world, dist, sample_clocks=True,
+                                                                 keep_last=bool(args.dump_outputs) and rank == 0)
+    if last_job is not None:
+        dump_outputs(last_job, args.dump_outputs)
+        last_job.close()
+        del last_job
+    nv_steps = args.steps
+    nv_s, nv_stats, _, _, _ = resident_arm(pkg, torch, ssts, handles, local_rank, stream_ptr, job_kw, 0, nv_steps, args.warmup, barrier, world, dist)
     launches = sum(s["gpu_kernel_launches"] for s in stats)
     out_bytes = stats[-1]["total_output_raw_key_bytes"] + stats[-1]["total_output_raw_value_bytes"]
     phases = [sum(s["phase_seconds"][i] for s in stats) / args.steps for i in range(5)]
@@ -513,7 +579,7 @@ def main():
             return st, data.size + meta.size
 
         def timed(step_fn, steps):
-            for _ in range(min(args.warmup, 2) if args.rows >= 50_000_000 else args.warmup):
+            for _ in range(args.warmup):
                 step_fn()
             for k in e2e_ms:
                 e2e_ms[k] = 0.0
@@ -527,7 +593,7 @@ def main():
                 dist.all_reduce(te, op=dist.ReduceOp.MAX)
             return float(te.item()), res
 
-        info_steps = max(1, min(args.steps, 5))          # the two informational modes; the headline runs args.steps
+        info_steps = args.steps
         e2e_s, res = timed(step_e2e, info_steps)
         single = {"value": round(in_bytes * world * info_steps / e2e_s / 1e9, 4), "unit": "GB/s", "steps": info_steps,
                   "h2d_bytes_per_step": int(res[-1][0]["h2d_bytes"]), "d2h_bytes_per_step": int(res[-1][0]["d2h_bytes"]),
@@ -652,8 +718,9 @@ def main():
                     sts.append(job.run().as_dict())
                     job.close()
                 return sts
-            c3_step()
-            c3_steps = 3
+            for _ in range(args.warmup):
+                c3_step()
+            c3_steps = args.steps
             barrier()
             t0 = time.perf_counter()
             c3_stats = [c3_step() for _ in range(c3_steps)]
@@ -690,12 +757,14 @@ def main():
                 kw4 = dict(job_kw, cutoff_ht=((c4.base_micros + 18 * 1000 + 500) << 12))
                 c4_in = sum(s_.raw_bytes for s_ in s4)
                 c4_entries = sum(s_.num_entries for s_ in s4)
-                c4_steps = 3
-                c4_s, c4_stats, _, _ = resident_arm(pkg, torch, s4, h4, local_rank, stream_ptr, kw4, args.verify, c4_steps, 1, barrier, world, dist)
+                c4_steps = args.steps
+                c4_s, c4_stats, _, _, _ = resident_arm(pkg, torch, s4, h4, local_rank, stream_ptr, kw4, args.verify, c4_steps, args.warmup,
+                                                       barrier, world, dist)
                 roof = pipeline_roofline(c4_stats, c4_in, hbm_peak, c4_steps)
                 extra["configs[3]"] = {
                     "workload": "MVCC-heavy: 20 versions/key, history_cutoff drops 90%%, %d live keys (%d entries, %.1f GB raw) resident on 1 GPU; "
-                                "BASELINE names 50M live keys = 1 G entries = 310 GB, which exceeds the 180 GB of HBM" % (live, c4_entries, c4_in / 1e9),
+                                "BASELINE names 50M live keys = 1 G entries = 310 GB, which exceeds the %.0f GiB of HBM" % (
+                                    live, c4_entries, c4_in / 1e9, props.total_memory / 2**30),
                     "value": round(c4_in * c4_steps / c4_s / 1e9, 2), "unit": "GB/s", "mkeys_per_s": round(c4_entries * c4_steps / c4_s / 1e6, 1),
                     "ms_per_step": round(c4_s / c4_steps * 1e3, 2), "steps": c4_steps, "entries": int(c4_entries),
                     "output_entries": int(c4_stats[-1]["num_output_records"]), "dropped_fraction": round(1.0 - c4_stats[-1]["num_output_records"] / c4_entries, 4),
@@ -755,28 +824,6 @@ def main():
     dom_kernel = max(kernel_s, key=lambda k: kernel_s[k])
     dom_bytes = kernel_alg[dom_kernel]
     achieved = dom_bytes / kernel_s[dom_kernel] / 1e9 if kernel_s[dom_kernel] > 0 else 0.0
-    # DRAM traffic of that kernel: NOT measured in this run — read from the committed `ncu --set full` capture of this
-    # same command (profiles/), labelled so
-    traffic, traffic_src = None, None
-    try:
-        if args.workload == "config2" and args.rows == DEFAULT_ROWS:
-            for fn in ("r02_ncu_full_100m.json", "r01_ncu_full_100m.json"):
-                path = os.path.join(ROOT, "profiles", fn)
-                if not os.path.exists(path):
-                    continue
-                prof = json.load(open(path))["kernels"]
-                want = {"ingest(verify+decode)": ("k_ingest", "k_decode"), "k_merge_filter": ("k_merge_filter",), "k_encode": ("k_encode",)}[dom_kernel]
-                for name, kd in prof.items():
-                    if name.startswith(want):
-                        def gb(x):
-                            v = float(x["value"]); return v * {"Gbyte": 1e9, "Mbyte": 1e6, "Kbyte": 1e3, "byte": 1.0}[x["unit"]]
-                        traffic = int(gb(kd["dram__bytes_read.sum"]) + gb(kd["dram__bytes_write.sum"]))
-                        traffic_src = "profiles/%s (%s), committed capture, not measured in this run" % (fn, name)
-                        break
-                if traffic is not None:
-                    break
-    except Exception:
-        traffic = None
     value = in_bytes * world * args.steps / total_s / 1e9
     line = {
         "metric": "compaction GB/s (input bytes merged)", "value": round(value, 3), "unit": "GB/s",
@@ -792,15 +839,16 @@ def main():
                    "verify_checksums": bool(args.verify),
                    "host_placement": {"numa_node": numa_node, "cpus": numa_cpus},
                    "output": "split SST: data blocks + CRC32C, multi-level index, DocKeyV3 bloom filter blocks (64 KB), properties, footer",
-                   "l2": "inputs (%.1f GB) far larger than the 126 MB L2" % (file_bytes / 1e9)},
+                   "l2": "inputs (%.1f GB) far larger than the %d MB L2" % (file_bytes / 1e9, props.L2_cache_size >> 20)},
         "mkeys_per_s": round(n_entries * world * args.steps / total_s / 1e6, 2),
         "gpu_launches": int(launches),
+        "gpu": {"name": props.name, "power_limit_w": (clock_info or {}).get("power_limit_w")},
         "clocks": clock_info,
         "value_no_verify": {"value": round(in_bytes * world * nv_steps / nv_s / 1e9, 3), "unit": "GB/s", "steps": nv_steps,
                             "ms_per_step": round(nv_s / nv_steps * 1e3, 3),
                             "note": "input block checksums NOT verified (work the reference does is skipped): informational only"},
         "roofline": {"bound": "hbm", "kernel": dom_kernel, "achieved": round(achieved, 1), "peak": hbm_peak, "unit": "GB/s",
-                     "frac": round(achieved / hbm_peak, 4), "traffic": traffic, "traffic_source": traffic_src, "peak_source": peak_kind,
+                     "frac": round(achieved / hbm_peak, 4), "peak_source": peak_kind,
                      "kernel_ms": round(kernel_s[dom_kernel] * 1e3, 3), "algorithmic_bytes_per_launch": int(dom_bytes),
                      "kernels_ms": {k: round(v * 1e3, 3) for k, v in kernel_s.items()},
                      "pipeline": pipeline_roofline(stats, in_bytes, hbm_peak, args.steps),
@@ -823,7 +871,7 @@ def config5_sharded(args, pkg, torch, dist, rank, world, local_rank, job_kw, hbm
     """BASELINE configs[4]: ONE oversized tablet, 32 input files, key-range sharded across the GPUs through
     ybgpu_compact_range_sharded (C++ over NCCL: splitters all-gathered, block slices exchanged with chunked grouped
     ncclSend / ncclRecv over NVLink, every rank compacting its key range). All ranks call this; returns the
-    sub-result on rank 0. Scaled: --c5-rows-per-gpu entries per GPU (the 1 TB of BASELINE does not fit 8 x 180 GB
+    sub-result on rank 0. Scaled: --c5-rows-per-gpu entries per GPU (the 1 TB of BASELINE does not fit 8 x 80 GB
     together with the outputs; the `rounds` mechanism that bounds HBM use is exercised by the tests)."""
     n_files = 32
     total_rows = args.c5_rows_per_gpu * world
@@ -848,9 +896,10 @@ def config5_sharded(args, pkg, torch, dist, rank, world, local_rank, job_kw, hbm
     dist.broadcast_object_list(uid, src=0)
     comm = pkg.RangeComm(uid[0], rank, world, local_rank)
     results = []
-    steps = 2
+    steps = args.steps
+    warm = max(1, args.warmup)                       # at least one warm-up: communicator set-up, allocator
     dts = []
-    for it in range(1 + steps):                      # one warm-up (communicator set-up, allocator) + `steps` timed
+    for it in range(warm + steps):
         barrier()
         t0 = time.perf_counter()
         data, meta, res, st = comm.compact(files, rounds=1, chunk_bytes=64 << 20, data_out=out_data, meta_out=out_meta,
@@ -860,7 +909,7 @@ def config5_sharded(args, pkg, torch, dist, rank, world, local_rank, job_kw, hbm
         dt = time.perf_counter() - t0
         te = torch.tensor([dt], dtype=torch.float64, device="cuda")
         dist.all_reduce(te, op=dist.ReduceOp.MAX)
-        if it:
+        if it >= warm:
             dts.append(float(te.item()))
             results.append((res, st))
     res, st = results[-1]

@@ -1,5 +1,5 @@
 /*
- * ybgpu_compaction.h — C ABI of the B200-native DocDB compaction engine.
+ * ybgpu_compaction.h — C ABI of the H100-native DocDB compaction engine.
  *
  * This is the drop-in boundary for the one hot path this repository replaces: the loop inside
  * rocksdb::CompactionJob::ProcessKeyValueCompaction (reference

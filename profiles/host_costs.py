@@ -5,7 +5,7 @@ pick row-aligned splitters) and the one-table assembly (ybgpu_sst_concat_meta). 
 of BASELINE config 2 (8 inputs, ~9.2e5 data blocks in total); data blocks are 4 KB here instead of 32 KB so
 that the files stay small. Needs no GPU.
 
-    python profiles/host_costs.py > profiles/r01_host_costs.json
+    python profiles/host_costs.py > host_costs.json
 """
 import importlib
 import json

@@ -1,7 +1,7 @@
-"""yugabyte-db_b200 — B200-native DocDB compaction engine.
+"""yugabyte-db_b200 — H100-native DocDB compaction engine.
 
 Python is only the test / bench binding over the C ABI in include/ybgpu_compaction.h (the product
-is libybgpu.so: hand-written sm_100a CUDA + a C++ host layer). Importing this package never
+is libybgpu.so: hand-written sm_90a CUDA + a C++ host layer). Importing this package never
 falls back to a CPU implementation: if libybgpu.so is missing the import fails loudly.
 """
 from .binding import (  # noqa: F401

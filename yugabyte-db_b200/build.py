@@ -1,4 +1,4 @@
-"""Builds libybgpu.so (sm_100a) in-tree with nvcc. Used by __graft_entry__.build()."""
+"""Builds libybgpu.so (sm_90a, H100) in-tree with nvcc. Used by __graft_entry__.build()."""
 import os
 import subprocess
 import sys
@@ -7,7 +7,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libybgpu.so")
 SOURCES = ["engine.cu", "abi.cc", "host_sst.cc", "host_gen.cc", "subcompaction.cc", "numa.cc", "range_exchange.cc"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC,-msse4.2,-Wall", "--shared", "-cudart", "shared", "-ldl"]
 
 

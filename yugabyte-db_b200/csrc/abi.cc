@@ -477,6 +477,6 @@ ybgpu_status ybgpu_sst_verify_blocks(const uint8_t* meta, uint64_t meta_len, con
 }
 
 int32_t ybgpu_device_count(void);   // engine.cu
-const char* ybgpu_version(void) { return "ybgpu-compaction 0.1 (sm_100a)"; }
+const char* ybgpu_version(void) { return "ybgpu-compaction 0.1 (sm_90a)"; }
 
 }  // extern "C"

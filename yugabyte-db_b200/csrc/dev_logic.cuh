@@ -1,6 +1,6 @@
-// dev_logic.cuh — per-entry device logic of the B200 compaction engine.
+// dev_logic.cuh — per-entry device logic of the H100 compaction engine.
 //
-// Everything here is __host__ __device__ so the same code that runs inside the sm_100a kernels
+// Everything here is __host__ __device__ so the same code that runs inside the sm_90a kernels
 // (engine.cu) can be unit-tested on the CPU by tests/host_harness (this container has no GPU).
 // The product never executes these functions on the host.
 //

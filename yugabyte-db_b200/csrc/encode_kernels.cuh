@@ -201,7 +201,7 @@ __global__ void __launch_bounds__(1024) k_scan_u64_single(unsigned long long* a,
   if (threadIdx.x == 0 && total) *total = carry;
 }
 // Exclusive scan of a long u64 array in place (block sizes -> file offsets): chunk sums, one-CTA scan of the chunk sums
-// (k_scan_u64_single), then every chunk scans itself from its base. (One CTA walking 10^6 elements took 0.9 ms.)
+// (k_scan_u64_single), then every chunk scans itself from its base.
 __global__ void __launch_bounds__(256) k_u64_chunk_sums(const unsigned long long* a, uint32_t n, unsigned long long* partial) {
   __shared__ unsigned long long sh;
   if (threadIdx.x == 0) sh = 0;
@@ -280,10 +280,6 @@ __device__ __forceinline__ unsigned long long blk_cur(const EncView& E, uint32_t
 }
 
 // next[s]: first entry of the block after the one starting at s (flush_block_policy.cc:45-76).
-// (A two-level variant — every 32nd start searched fully, the others guided by their neighbour's block
-// length — measured slower on B200 than this single pass from a static guess and was dropped.)
-// (Staging the P / QQ window of 1024 consecutive starts in shared memory measured slower, 4.5 vs 4.1 ms at 10^8 entries:
-// the probes hit L2 anyway and the staging halves the occupancy.)
 __global__ void __launch_bounds__(256) k_next(EncView E) {
   const unsigned long long BS = E.block_size;
   const unsigned long long thresh = BS * (100 - E.deviation);       // cur*100 > thresh
@@ -1601,9 +1597,8 @@ __global__ void __launch_bounds__(ENC5_THREADS, ENC == 1 ? 4 : 2) k_encode_v5(En
         }
       }
       if (next_val) {
-        // (whole values: ~39 MB of requested lines are in flight across the GPU and ncu shows 11 GB more DRAM reads per
-        // 10^8 entries than without — lines evicted before use — but requesting only each value's first line measured
-        // 5 % slower: the kernel is bound by latency, not by bandwidth)
+        // (whole values: some requested lines are evicted before use, but the kernel is bound by latency, not by
+        // bandwidth)
         const uint32_t vl = d_next.vlen_out;
         for (uint32_t o = 0; o < vl; o += 128) enc5_prefetch_l2(next_val + o);
         if (vl) enc5_prefetch_l2(next_val + vl - 1);

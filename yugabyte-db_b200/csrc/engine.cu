@@ -1,4 +1,4 @@
-// engine.cu — B200 (sm_100a) DocDB compaction engine: kernels + host orchestration.
+// engine.cu — H100 (sm_90a) DocDB compaction engine: kernels + host orchestration.
 //
 // Pipeline (one ybgpu_job = one rocksdb::CompactionJob::Run, reference
 // src/yb/rocksdb/db/compaction_job.cc:664-895):
@@ -1538,7 +1538,7 @@ constexpr size_t STATUS_READ_BYTES = 4096;             // [0, 4096): read-backs;
 constexpr size_t STATUS_PAGE_BYTES = 65536;
 struct StatusPage { uint8_t* host = nullptr; uint8_t* dev = nullptr; };
 static std::mutex g_status_mu;
-static std::vector<StatusPage> g_status_free;          // process-wide: cudaHostAlloc costs ~1 ms
+static std::vector<StatusPage> g_status_free;          // process-wide: cudaHostAlloc is expensive
 static cudaError_t AcquireStatusPage(StatusPage* p) {
   {
     std::lock_guard<std::mutex> lock(g_status_mu);
@@ -1695,7 +1695,7 @@ ybgpu_status Engine::Init() {
     CUDA_TRY(cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &thr));
     // Never satisfy an allocation with memory whose free is still pending on ANOTHER stream: the pool would make this
     // job's stream wait for that stream's queued work — in a pipelined compaction that is a neighbour's multi-GB output
-    // copy, and this job's kernels would sit behind it (seen as 50-80 ms "run" phases of 5 ms jobs). Memory whose free
+    // copy, and this job's kernels would sit behind it. Memory whose free
     // has completed is still reused; otherwise the pool grows.
     int off = 0;
     CUDA_TRY(cudaMemPoolSetAttribute(pool, cudaMemPoolReuseAllowInternalDependencies, &off));
@@ -2305,7 +2305,6 @@ ybgpu_status Engine::Run(const volatile int32_t* shutting_down) {
     if (ybgpu_status us = UploadSmall(d_sample_base, sample_base.data(), 4 * (k + 1))) return us;
     CUDA_TRY(cudaMemsetAsync(pv.bucket_min, 0xff, static_cast<size_t>(n_buckets) * 8, I.stream));
     pv.runs = I.dRuns; pv.sample_base = d_sample_base; pv.n_samples = n_samples; pv.n_buckets = n_buckets;
-    // (one thread per sample looping over the runs measured slower than one thread per (sample, run): 6.0 vs ~5 ms)
     k_sample_pos<<<GridFor(static_cast<uint64_t>(n_samples) * k, 256, sms), 256, 0, I.stream>>>(pv, I.dP, I.dJ, 0);
     k_sample_pos<<<GridFor(static_cast<uint64_t>(n_samples) * k, 256, sms), 256, 0, I.stream>>>(pv, I.dP, I.dJ, 1);
     k_sample_bucket<<<GridFor(n_samples, 256, sms), 256, 0, I.stream>>>(pv, I.dP);
@@ -2823,8 +2822,10 @@ ybgpu_status Engine::Digest(uint64_t* digest) {
   if (ybgpu_status s = EnsureKvStream()) return s;
   Impl& I = *impl_;
   CUDA_TRY(cudaSetDevice(opt_.device));
+  int sms = 0;
+  CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, opt_.device));
   CUDA_TRY(cudaMemsetAsync(&I.dJ->digest, 0, 8, I.stream));
-  if (I.n_out) k_digest<<<GridFor(I.n_out, 256, 148), 256, 0, I.stream>>>(I.out_keys, I.out_koff, I.out_vals, I.out_voff, I.n_out, I.dJ);
+  if (I.n_out) k_digest<<<GridFor(I.n_out, 256, sms), 256, 0, I.stream>>>(I.out_keys, I.out_koff, I.out_vals, I.out_voff, I.n_out, I.dJ);
   CUDA_TRY(cudaGetLastError());
   CUDA_TRY(cudaMemcpyAsync(&I.hJ, I.dJ, sizeof(JobDev), cudaMemcpyDeviceToHost, I.stream));
   CUDA_TRY(cudaStreamSynchronize(I.stream));

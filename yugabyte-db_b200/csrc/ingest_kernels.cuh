@@ -178,8 +178,7 @@ struct IngEntry { uint16_t estart, kstart, vstart, vlen, shared, klen; };    // 
 //   word address of T_t[e], copy c  =  e * 32 + t * 8 + c        (bank = t * 8 + c, independent of e)
 // A lane uses copy (lane & 7) and looks the four bytes of a word step up in ROTATED order: in its k-th look-up it
 // addresses table t = (k + (lane >> 3)) & 3. The 32 lanes of a warp then hit 32 different banks in every one of the
-// four look-up instructions, whatever the data: no bank conflicts with 32 KB of tables (the plain interleaved layout
-// with 8 copies measured 2.4 wavefronts per look-up, ncu r02_ncu_full_100m_v1).
+// four look-up instructions, whatever the data: no bank conflicts with 32 KB of tables.
 struct IngTab {
   const uint32_t* base;            // table words in shared memory
   uint32_t sel[4];                 // PRMT selector extracting the byte table t_k consumes (T3 <-> byte 0 ... T0 <-> byte 3)
@@ -446,10 +445,7 @@ __global__ void __launch_bounds__(ING_THREADS, 2) k_ingest(IngestView V, JobDev*
         // the block's entry count was fixed by the probe + scan; it must agree with what the walk found
         else if (n_ent != expect) { dev_fail(J, DEV_ERR_IRREGULAR_RESTARTS, b); n_ent = 0; }
         // (the CRC of the block's tail is left to the CRC warps: this warp is the serial stage of the pipeline — a lane
-        // parses its restart interval entry by entry — and what it does beyond that lengthens the pipeline period. Measured:
-        // building previous-smaller links here cost 3.3 ms per 10^8 entries, moving the tail CRC out gained 2.3 ms; moving
-        // validation and the entry table to the consumer warps as well gained nothing — the consumers then re-parse every
-        // header and the kernel, at 62 % issue utilisation, is bound by its instruction count.)
+        // parses its restart interval entry by entry — and what it does beyond that lengthens the pipeline period.)
         sh_nent[stage] = n_ent; sh_tail[stage] = tail;
       }
       __syncwarp();                                // the lanes' entry table writes are ordered before lane 0's arrive
