@@ -1506,7 +1506,9 @@ __global__ void __launch_bounds__(ENC5_THREADS, ENC == 1 ? 4 : 2) k_encode_v5(En
     unsigned long long acc = 0;                  // XOR of unreduced carry-less products
     // The kernel is bound by memory latency (a round's loads form a chain: descriptor -> record / value offset -> value
     // bytes), so the next round's chain is started ahead: its descriptors are loaded while this round's entries are
-    // assembled, its record and value lines are requested into L2 while this round's values are copied.
+    // assembled, its record lines are requested into L2 while this round's values are copied. Its value lines are not:
+    // with every warp of the machine asking for the next 32 values (~43 MB ahead, most of the 50 MB L2, which also holds
+    // the lines being written) part of them was evicted before use and read from DRAM twice (DESIGN.md §4).
     Desc d_cur{};
     if (s + lane < e) d_cur = E.kept[s + lane];
     for (uint32_t r0 = s; r0 < e; r0 += 32) {
@@ -1559,12 +1561,9 @@ __global__ void __launch_bounds__(ENC5_THREADS, ENC == 1 ? 4 : 2) k_encode_v5(En
         }
       }
       __syncwarp();
-      const uint8_t* next_val = nullptr;
       if (jn < e) {
         const RunView& rn = E.runs[d_next.run];
-        const uint32_t idxn = d_next.gid - rn.gid_base;
-        enc5_prefetch_l2(rn.rec + static_cast<size_t>(idxn) * S);
-        next_val = rn.data + rn.val_off[idxn];
+        enc5_prefetch_l2(rn.rec + static_cast<size_t>(d_next.gid - rn.gid_base) * S);
       }
       const uint32_t nact = min(32u, e - r0);
 #pragma unroll 2
@@ -1595,13 +1594,6 @@ __global__ void __launch_bounds__(ENC5_THREADS, ENC == 1 ? 4 : 2) k_encode_v5(En
             for (uint32_t i = hl; i < len_q; i += 16) vd[i] = __ldg(src + i);
           }
         }
-      }
-      if (next_val) {
-        // (whole values: some requested lines are evicted before use, but the kernel is bound by latency, not by
-        // bandwidth)
-        const uint32_t vl = d_next.vlen_out;
-        for (uint32_t o = 0; o < vl; o += 128) enc5_prefetch_l2(next_val + o);
-        if (vl) enc5_prefetch_l2(next_val + vl - 1);
       }
       d_cur = d_next;
       __syncwarp();                                // the scratch rows are rewritten by the next round
