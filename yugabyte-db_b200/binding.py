@@ -77,6 +77,8 @@ class JobStats(C.Structure):
 PHASE_NAMES = ["block_scan", "decode", "partition", "merge_filter", "encode"]
 PATH_FUSED_INGEST, PATH_GENERAL_DECODE, PATH_SNAPPY, PATH_PARTITION_RETRY, PATH_ENCODER_V4, PATH_ENCODER_V5, PATH_KV_INPUT = 1, 2, 4, 8, 16, 32, 64
 PATH_SNAPPY_OUTPUT = 128
+PATH_LZ4, PATH_LZ4_OUTPUT = 256, 512
+COMPRESSION_NONE, COMPRESSION_SNAPPY, COMPRESSION_LZ4 = 0, 1, 4   # output_compression (rocksdb::CompressionType)
 
 
 class GenConfig(C.Structure):

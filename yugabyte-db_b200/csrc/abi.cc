@@ -69,6 +69,9 @@ void ybgpu_job_options_init(ybgpu_job_options* o) {
 
 ybgpu_status ybgpu_job_create(const ybgpu_job_options* options, ybgpu_job** job) {
   if (!options || !job) { g_last_error = "null argument"; return YBGPU_INVALID_ARGUMENT; }
+  if (!ybgpu::host::OutputCompressionSupported(options->output_compression)) {
+    g_last_error = ybgpu::host::UnsupportedOutputCompression(options->output_compression); return YBGPU_NOT_SUPPORTED;
+  }
   std::unique_ptr<ybgpu_job> j(new ybgpu_job);
   j->engine.reset(new Engine(*options));
   ybgpu_status s = j->engine->Init();
@@ -332,6 +335,9 @@ struct ybgpu_table_builder {
 
 ybgpu_status ybgpu_table_builder_create(const ybgpu_job_options* o, ybgpu_table_builder** b) {
   if (!o || !b) return YBGPU_INVALID_ARGUMENT;
+  if (!ybgpu::host::OutputCompressionSupported(o->output_compression)) {
+    g_last_error = ybgpu::host::UnsupportedOutputCompression(o->output_compression); return YBGPU_NOT_SUPPORTED;
+  }
   try {
     ybgpu::host::TableOptions t;
     t.block_size = o->block_size; t.block_restart_interval = o->block_restart_interval;
@@ -429,12 +435,32 @@ ybgpu_status ybgpu_sst_concat_meta(const ybgpu_job_options* o, const ybgpu_sst_p
   return YBGPU_OK;
 }
 
+}  // extern "C"
+
+// Whether the first bytes of a block labelled LZ4 / LZ4HC can open a stream the engine decodes: a varint32 preamble
+// below k_snappy_sizes' 2^30 limit, then a raw LZ4 block, which is exactly one byte (an empty token) when the announced
+// length is 0 and longer otherwise (a non-empty output needs a token and its literals). Reads at most 5 bytes.
+static bool Lz4PreambleFits(const uint8_t* p, uint64_t n) {
+  uint64_t u = 0;
+  for (uint64_t i = 0; i < 5 && i < n; i++) {
+    u |= static_cast<uint64_t>(p[i] & 127) << (7 * i);
+    if (!(p[i] & 128)) {
+      const uint64_t body = n - i - 1;
+      return u < (1u << 30) && body >= 1 && (u == 0) == (body == 1);
+    }
+  }
+  return false;
+}
+
+extern "C" {
+
 ybgpu_status ybgpu_sst_check_supported(const uint8_t* meta, uint64_t meta_len, const uint8_t* data, uint64_t data_len, uint64_t counts[8]) {
   if (!meta || (!data && data_len)) { g_last_error = "null argument"; return YBGPU_INVALID_ARGUMENT; }
   ybgpu::host::SstMeta m;
   std::string err = ybgpu::host::ParseSplitSstMeta(meta, meta_len, &m);
   if (!err.empty()) { g_last_error = err; return YBGPU_CORRUPTION; }
   uint64_t local[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+  uint64_t lz4_unfit = 0;                                   // blocks labelled LZ4 whose first bytes open no LZ4 stream
   for (const ybgpu::host::Handle& h : m.data_blocks) {
     if (h.offset > data_len || h.size > data_len - h.offset || data_len - h.offset - h.size < 5) {
       g_last_error = "a data block handle points outside the data file"; return YBGPU_CORRUPTION;
@@ -442,17 +468,23 @@ ybgpu_status ybgpu_sst_check_supported(const uint8_t* meta, uint64_t meta_len, c
     const uint8_t type = data[h.offset + h.size];
     if (type > 7) { g_last_error = "unknown block compression type " + std::to_string(type); return YBGPU_CORRUPTION; }
     local[type]++;
+    if ((type == 4 || type == 5) && !Lz4PreambleFits(data + h.offset, h.size)) lz4_unfit++;
   }
   if (counts) memcpy(counts, local, sizeof(local));
   if (m.key_encoding != YBGPU_KEY_ENCODING_SHARED_PREFIX && m.key_encoding != YBGPU_KEY_ENCODING_THREE_SHARED_PARTS) {
     g_last_error = "data block key-value encoding format " + std::to_string(m.key_encoding) + " is not decoded by the engine"; return YBGPU_NOT_SUPPORTED;
   }
   for (int t = 2; t < 8; t++)
-    if (local[t]) {
+    if (local[t] && t != 4 && t != 5) {
       static const char* const kNames[8] = {"none", "snappy", "zlib", "bzip2", "lz4", "lz4hc", "xpress", "zstd"};
-      g_last_error = std::to_string(local[t]) + " data blocks are stored with " + kNames[t] + " compression: only raw and Snappy blocks are decoded on the GPU";
+      g_last_error = std::to_string(local[t]) + " data blocks are stored with " + kNames[t] +
+                     " compression: only raw, Snappy and LZ4 (LZ4HC) blocks are decoded on the GPU";
       return YBGPU_NOT_SUPPORTED;
     }
+  if (lz4_unfit) {
+    g_last_error = std::to_string(lz4_unfit) + " data blocks labelled LZ4 do not start with an LZ4 length preamble the engine decodes";
+    return YBGPU_NOT_SUPPORTED;
+  }
   return YBGPU_OK;
 }
 
@@ -470,7 +502,8 @@ ybgpu_status ybgpu_sst_verify_blocks(const uint8_t* meta, uint64_t meta_len, con
     if (h.offset + h.size + 5 > data_len) { (*bad)++; continue; }
     const uint8_t* p = data + h.offset;
     uint32_t stored; memcpy(&stored, p + h.size + 1, 4);
-    if (p[h.size] > 1 /* kNoCompression / kSnappyCompression: the checksum covers the stored bytes */ || ybgpu::host::Crc32cMask(ybgpu::host::Crc32c(p, h.size + 1)) != stored) (*bad)++;
+    const uint8_t type = p[h.size];                        // none, Snappy, LZ4, LZ4HC: the checksum covers the stored bytes
+    if ((type > 1 && type != 4 && type != 5) || ybgpu::host::Crc32cMask(ybgpu::host::Crc32c(p, h.size + 1)) != stored) (*bad)++;
   }
   if (*bad) { g_last_error = "block checksum mismatch"; return YBGPU_CORRUPTION; }
   return YBGPU_OK;

@@ -100,8 +100,14 @@ __global__ void __launch_bounds__(256) k_restart_probe(const RunView* runs, cons
     uint32_t nres = size >= 4 ? ldg_u32_unaligned(blk + size - 4) : 0;
     const uint8_t type = blk[size];                        // trailer: compression type of the stored block
     if (type != 0) {
-      // Snappy blocks are uncompressed by the host's next stage (snappy_kernels.cuh), then the probe runs again
-      if (type == 1) atomicAdd(&J->n_compressed, 1u); else dev_fail(J, DEV_ERR_COMPRESSED, b);
+      // Snappy and LZ4 (LZ4HC) blocks are uncompressed by the host's next stage (snappy_kernels.cuh, lz4_kernels.cuh),
+      // then the probe runs again
+      if (type == 1 || type == 4 || type == 5) {
+        atomicAdd(&J->n_compressed, 1u);
+        if (type != 1) atomicAdd(&J->n_lz4, 1u);
+      } else {
+        dev_fail(J, DEV_ERR_COMPRESSED, b);
+      }
       nres = 0;
     } else if (nres == 0 || static_cast<uint64_t>(nres) * 4 + 4 > size) { dev_fail(J, DEV_ERR_BAD_BLOCK, b); nres = 0; }
     if (nres == 0) continue;

@@ -211,6 +211,8 @@ ybgpu_status ybgpu_compact_range_sharded(ybgpu_range_comm* c, const ybgpu_job_op
     if (err && err_cap) snprintf(err, err_cap, "%s", msg.c_str());
     return s;
   };
+  if (options && !ybgpu::host::OutputCompressionSupported(options->output_compression))
+    return fail(YBGPU_NOT_SUPPORTED, ybgpu::host::UnsupportedOutputCompression(options->output_compression));
   std::string nerr;
   const NcclApi* N = Nccl(&nerr);
   if (!N) return fail(YBGPU_RUNTIME_ERROR, nerr);

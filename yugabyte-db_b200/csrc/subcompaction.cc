@@ -230,12 +230,11 @@ bool LastKeyOfFile(const ybgpu_input_file& f, const SstMeta& m, std::string* key
     if (ybgpu::host::Crc32cMask(ybgpu::host::Crc32c(p, h.size + 1)) != stored) return false;
   }
   const uint8_t type = f.data_file[h.offset + h.size];
-  if (type == 1) {                                                  // Snappy (the production default): uncompress on the host
+  if (type != 0) {                                                  // stored compressed: uncompress on the host
     std::string raw;
-    if (!ybgpu::host::SnappyUncompressBlock(f.data_file + h.offset, h.size, &raw)) return false;
+    if (!ybgpu::host::UncompressStoredBlock(type, f.data_file + h.offset, h.size, &raw)) return false;
     return LastKeyOfBlock(reinterpret_cast<const uint8_t*>(raw.data()), raw.size(), m.key_encoding, key);
   }
-  if (type != 0) return false;                                      // other codecs: not supported
   return LastKeyOfBlock(f.data_file + h.offset, h.size, m.key_encoding, key);
 }
 
@@ -322,6 +321,8 @@ ybgpu_status CompactFilesCore(const ybgpu_job_options* options, const ybgpu_inpu
   };
   if (!options || !files || !outputs || !num_outputs || !data_arena || (!meta_arena && !one)) return fail(YBGPU_INVALID_ARGUMENT, "null argument");
   if (options->range_lower_len || options->range_upper_len) return fail(YBGPU_INVALID_ARGUMENT, "range bounds are set by the subcompaction planner");
+  if (!ybgpu::host::OutputCompressionSupported(options->output_compression))
+    return fail(YBGPU_NOT_SUPPORTED, ybgpu::host::UnsupportedOutputCompression(options->output_compression));
   if (max_subcompactions == 0) max_subcompactions = 1;
   if (max_in_flight == 0) max_in_flight = 3;
   std::vector<ParsedInput> in;
