@@ -51,8 +51,8 @@ enum DevError : int {
   DEV_ERR_STACK_DEPTH = 11,       // more subkey levels than DEV_MAX_DEPTH
   DEV_ERR_UNSUPPORTED_VALUE = 12, // packed rows (need SchemaPackingProvider), merge/single-delete types
   DEV_ERR_BAD_CRC = 13,
-  DEV_ERR_COTABLE = 14,           // cotable / colocation ids: table-tombstone carry not implemented
-  DEV_ERR_SHORT_KEY = 15,         // internal key shorter than 8 bytes
+  // 14 is retired: it was the per-tile limit on cotable / colocated tables, which no longer exists
+  DEV_ERR_SHORT_KEY = 15,        // internal key shorter than 8 bytes
   DEV_ERR_UNSORTED = 16,          // input run not sorted
 };
 
@@ -1121,54 +1121,96 @@ YB_HD uint32_t replay_lower_bound(const ReplayRun& run, int S, const uint8_t* ke
   return lo;
 }
 
+// One entry of a replay, in merged order: rule A against the entry replayed before it (*prev), deletions that are
+// obsolete at the bottommost level skipped, every other entry fed. `val` = the value, needed only when its first byte
+// announces control fields (nullptr otherwise). Returns 0 or a negative DevError.
+YB_HD int replay_entry(FeedState* st, const RetentionDev& R, const uint8_t* rec, int S, const uint8_t* val,
+                       const uint8_t** prev, int bottommost, uint64_t last_sequence) {
+  const uint32_t cl = rec_ulen(rec, S);
+  const bool hidden = *prev && cmp_user_keys(*prev, rec_ulen(*prev, S), rec, cl) == 0;   // rule A
+  *prev = rec;
+  if (hidden) return 0;
+  const uint64_t suffix = rec_suffix(rec, S);
+  if ((suffix & 0xff) == 0 && bottommost && (suffix >> 8) <= last_sequence) return 0;    // obsolete deletion
+  ValueRewrite rw;
+  const int d = feed_step(st, R, rec, cl, rec_vfirst(rec, S), val, rec_vlen(rec, S), &rw);
+  return d < 0 ? d : 0;
+}
+
+// Replays, in merged order, the entries below runs[r].limit whose user key starts with key[0, g) + '#', except those
+// whose flags intersect `skip`. The entries of one pattern are contiguous in every run: one galloping search per run,
+// then a k-way merge of the k cursors. Returns 0 or a negative DevError.
+YB_HD_NOINLINE int replay_pattern(FeedState* st, const RetentionDev& R, const ReplayRun* runs, int k, int S,
+                                  const uint8_t* key, uint32_t g, uint8_t skip, int bottommost, uint64_t last_sequence) {
+  uint32_t cur[REPLAY_MAX_RUNS];
+  for (int r = 0; r < k; r++) cur[r] = replay_lower_bound(runs[r], S, key, g);
+  const uint8_t* prev = nullptr;
+  for (;;) {
+    int best = -1; const uint8_t* bk = nullptr;
+    for (int r = 0; r < k; r++) {
+      if (cur[r] >= runs[r].limit) continue;
+      const uint8_t* c = runs[r].rec + static_cast<size_t>(cur[r]) * S;
+      if (cmp_pattern(key, g, '#', c, rec_ulen(c, S)) != 0) { cur[r] = runs[r].limit; continue; }   // left the pattern
+      if (best < 0 || cmp_records(c, bk, S) < 0) { best = r; bk = c; }
+    }
+    if (best < 0) break;
+    const uint32_t idx = cur[best]++;
+    if (rec_flags(bk, S) & skip) continue;
+    const uint8_t* val = nullptr;
+    if (rec_vlen(bk, S) && has_control_fields(rec_vfirst(bk, S))) val = runs[best].data + runs[best].val_off[idx];
+    const int d = replay_entry(st, R, bk, S, val, &prev, bottommost, last_sequence);
+    if (d < 0) return d;
+  }
+  return 0;
+}
+
 // Brings *st (freshly reset, or seeded with the table tombstone state of a cotable) to the state Feed has
 // when it reaches the record k0, which is the first record of a tile and lies inside a row group that
 // began in an earlier tile. runs[r].limit = index of the first record of run r that belongs to this tile
 // or a later one (everything below it sorts before k0). Returns 0 or a negative DevError.
 YB_HD_NOINLINE int replay_ancestors(FeedState* st, const RetentionDev& R, const ReplayRun* runs, int k, int S,
                                     const uint8_t* k0, uint32_t ulen0, int bottommost, uint64_t last_sequence) {
-  if (k > REPLAY_MAX_RUNS) return -DEV_ERR_COTABLE;
   uint32_t ends[DEV_MAX_DEPTH];
   const int n = decode_key_ends(k0, ulen0, ends);
   if (n < 0) return n;
   const uint8_t t0 = k0[0];
   const bool sub_doc_key = !(t0 == 6 || t0 == 7);
   // level 0 of a SubDocKey is the table id: its entries are the table tombstones `id ! # HT`, which seed the rows
-  // of the table elsewhere (cotable seeding). Only when k0 is itself such a tombstone are its earlier versions
-  // replayed here: their pattern is id + '!' + '#'.
+  // of the table elsewhere (table_seed / replay_table_seed). Only when k0 is itself such a tombstone are its earlier
+  // versions replayed here: their pattern is id + '!' + '#'.
   const bool tombstone = sub_doc_key && n == 1;
   for (int lev = (sub_doc_key && !tombstone) ? 1 : 0; lev < n; lev++) {
     const uint32_t g = tombstone ? ends[0] + 1 : ends[lev];
     if (g >= ulen0) break;
-    uint32_t cur[REPLAY_MAX_RUNS];
-    for (int r = 0; r < k; r++) cur[r] = replay_lower_bound(runs[r], S, k0, g);
-    const uint8_t* prev = nullptr;
-    for (;;) {
-      int best = -1; const uint8_t* bk = nullptr;
-      for (int r = 0; r < k; r++) {
-        if (cur[r] >= runs[r].limit) continue;
-        const uint8_t* c = runs[r].rec + static_cast<size_t>(cur[r]) * S;
-        if (cmp_pattern(k0, g, '#', c, rec_ulen(c, S)) != 0) { cur[r] = runs[r].limit; continue; }   // left the level
-        if (best < 0 || cmp_records(c, bk, S) < 0) { best = r; bk = c; }
-      }
-      if (best < 0) break;
-      const uint32_t idx = cur[best]++;
-      if (rec_flags(bk, S) & REC_F_INVISIBLE) continue;
-      const uint32_t cl = rec_ulen(bk, S);
-      const bool hidden = prev && cmp_user_keys(prev, rec_ulen(prev, S), bk, cl) == 0;     // rule A
-      prev = bk;
-      if (hidden) continue;
-      const uint64_t suffix = rec_suffix(bk, S);
-      if ((suffix & 0xff) == 0 && bottommost && (suffix >> 8) <= last_sequence) continue;  // obsolete deletion
-      const uint32_t vlen = rec_vlen(bk, S);
-      const uint8_t vfirst = rec_vfirst(bk, S);
-      const uint8_t* val = nullptr;
-      if (vlen && has_control_fields(vfirst)) val = runs[best].data + runs[best].val_off[idx];
-      ValueRewrite rw;
-      const int d = feed_step(st, R, bk, cl, vfirst, val, vlen, &rw);
-      if (d < 0) return d;
-    }
+    const int d = replay_pattern(st, R, runs, k, S, k0, g, REC_F_INVISIBLE, bottommost, last_sequence);
+    if (d < 0) return d;
   }
+  return 0;
+}
+
+// Cotable / colocated tables. The table tombstones `id ! # HT` sort before every row of their table and form one row
+// group; Feed's slot 0 (the table-level overwrite) survives the row changes that follow (docdb_compaction_context.cc:
+// 999-1024). After the tombstones of a table were replayed on a fresh *st (rule A, bottommost obsolete deletions
+// skipped, HybridTime-filtered entries skipped, out-of-range ones INCLUDED: a key-range job that starts inside the
+// table loads them for exactly this), table_seed turns *st into the state every row of the table starts from: slot 0
+// kept (feed_state_seed) when the replay left a table-level overwrite, a reset state otherwise. `row` = a row key of
+// the table, `id` = its id length.
+YB_HD void table_seed(FeedState* st, const uint8_t* row, uint32_t id) {
+  if (st->n_ow >= 1 && st->n_ends == 1) feed_state_seed(st, row, id, st->ow[0]);
+  else feed_state_reset(st);
+}
+
+// The table tombstones of the table of `row` (id length `id`) replayed from the runs, below their limits, into *st,
+// which then holds the state the table's rows start from (table_seed). Returns 0 or a negative DevError.
+YB_HD_NOINLINE int replay_table_seed(FeedState* st, const RetentionDev& R, const ReplayRun* runs, int k, int S,
+                                     const uint8_t* row, uint32_t id, int bottommost, uint64_t last_sequence) {
+  alignas(8) uint8_t pattern[24] = {};                 // id + '!', zero padded (the id is 5 or 17 bytes)
+  for (uint32_t q = 0; q < id; q++) pattern[q] = row[q];
+  pattern[id] = '!';
+  feed_state_reset(st);
+  const int d = replay_pattern(st, R, runs, k, S, pattern, id + 1, REC_F_HT_FILTERED, bottommost, last_sequence);
+  if (d < 0) return d;
+  table_seed(st, row, id);
   return 0;
 }
 

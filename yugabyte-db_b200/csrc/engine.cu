@@ -634,9 +634,6 @@ struct MergeView {
 constexpr int MERGE_THREADS = 256;
 constexpr uint8_t ENT_GROUP_START = 128;           // tile-local: first entry of a row group (never leaves the merge kernel)
 constexpr uint32_t RW_PRE_DROPPED = 0xfffffffeu;   // rw_slot marker: dropped as an overwritten older version
-constexpr int COT_CAND_MAX = 16; // first row groups of id runs per tile (>= distinct ids)
-constexpr int COT_MAX = 8;       // distinct cotable / colocation ids per tile
-constexpr int COT_TOMB_MAX = 16; // table-tombstone entries replayed per id
 constexpr int RANK_C = 8;        // coarse stride of the two-level rank search
 constexpr int RANK_KMAX = 16;    // two-level search used for k <= RANK_KMAX runs
 
@@ -666,13 +663,81 @@ __host__ __device__ constexpr uint32_t bytes(uint32_t S, uint32_t cap) { return 
 }  // namespace tile_layout
 
 
+static_assert(MAX_RUNS <= REPLAY_MAX_RUNS, "a replay's cursors cover every run of a job");
+
 // One thread, rare: the run table for replay_ancestors lives in this function's frame, not in the kernel's.
 __device__ __noinline__ int seed_continuation(FeedState* st, const JobParams* prm, const RunView* runs, const uint32_t* seg_lo, int k, int S,
                                               const uint8_t* k0_smem) {
-  if (k > REPLAY_MAX_RUNS) return -DEV_ERR_COTABLE;
   ReplayRun rr[REPLAY_MAX_RUNS];
   for (int r = 0; r < k; r++) { rr[r].rec = runs[r].rec; rr[r].limit = seg_lo[r]; rr[r].data = runs[r].data; rr[r].val_off = runs[r].val_off; }
   return replay_ancestors(st, prm->R, rr, k, S, k0_smem, rec_ulen(k0_smem, S), prm->bottommost, prm->last_sequence);
+}
+
+// Id length of a cotable ('y') / colocated ('0') key, 0 for any other key (the key was validated by group_prefix_len).
+__device__ __forceinline__ int table_id_len(const uint8_t* e, uint32_t ulen) {
+  return (e[0] == 'y' || e[0] == '0') ? dockey_id_size(e, ulen) : 0;
+}
+
+// The one table of a tile whose tombstones may lie outside it: the table of the tile's first record. One thread, at
+// most once per tile: slot 0 of that table's rows from its tombstones in the runs — below the tile, or up to the tile's
+// end when the tile starts inside the tombstone group (`through_tile`). Returns 1 when the rows start from the
+// table-level overwrite *ow0, 0 when they start fresh, or a negative DevError.
+__device__ __noinline__ int seed_table_from_runs(Overwrite* ow0, const JobParams* prm, const RunView* runs, const uint32_t* seg_lo,
+                                                 const uint32_t* seg_start, int k, int S, const uint8_t* row, int id, bool through_tile) {
+  ReplayRun rr[REPLAY_MAX_RUNS];
+  for (int r = 0; r < k; r++) {
+    rr[r].rec = runs[r].rec; rr[r].data = runs[r].data; rr[r].val_off = runs[r].val_off;
+    rr[r].limit = seg_lo[r] + (through_tile ? seg_start[r + 1] - seg_start[r] : 0u);
+  }
+  FeedState st;
+  const int d = replay_table_seed(&st, prm->R, rr, k, S, row, static_cast<uint32_t>(id), prm->bottommost, prm->last_sequence);
+  if (d < 0) return d;
+  if (!st.n_ow) return 0;
+  *ow0 = st.ow[0];
+  return 1;
+}
+
+// Every other table of the tile: its tombstone group, sorted positions [i0, i1), is in shared memory. A row group of the
+// table replays it on *st (fresh) and turns the result into its starting state (table_seed).
+__device__ __noinline__ int seed_table_in_tile(FeedState* st, const JobParams* prm, const RunView* runs, const uint8_t* recs, int SS, int S,
+                                               const uint16_t* order, const uint32_t* seg_lo, const uint32_t* seg_start,
+                                               uint32_t i0, uint32_t i1, const uint8_t* row, int id) {
+  feed_state_reset(st);
+  const uint8_t* prev = nullptr;
+  for (uint32_t i = i0; i < i1; i++) {
+    const uint32_t li = order[i];
+    const uint8_t* c = recs + static_cast<size_t>(SS) * li;
+    if (rec_flags(c, S) & REC_F_HT_FILTERED) continue;           // out-of-range tombstones DO seed the table state
+    const uint8_t* val = nullptr;
+    if (rec_vlen(c, S) && has_control_fields(rec_vfirst(c, S))) {
+      int r = 0;
+      while (seg_start[r + 1] <= li) r++;
+      val = runs[r].data + runs[r].val_off[seg_lo[r] + (li - seg_start[r])];
+    }
+    const int d = replay_entry(st, prm->R, c, S, val, &prev, prm->bottommost, prm->last_sequence);
+    if (d < 0) return d;
+  }
+  table_seed(st, row, static_cast<uint32_t>(id));
+  return 0;
+}
+
+// Exclusive max-scan of one value per thread (0 for thread 0); all threads must call.
+__device__ __forceinline__ uint32_t block_exclusive_max(uint32_t v, uint32_t* warp_sums) {
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  uint32_t x = v;
+  for (int o = 1; o < 32; o <<= 1) { const uint32_t y = __shfl_up_sync(0xffffffffu, x, o); if (lane >= o) x = max(x, y); }
+  uint32_t ex = __shfl_up_sync(0xffffffffu, x, 1);
+  if (lane == 0) ex = 0;
+  __syncthreads();
+  if (lane == 31) warp_sums[wid] = x;
+  __syncthreads();
+  if (wid == 0) {
+    uint32_t m = lane < (blockDim.x >> 5) ? warp_sums[lane] : 0;
+    for (int o = 1; o < 32; o <<= 1) { const uint32_t y = __shfl_up_sync(0xffffffffu, m, o); if (lane >= o) m = max(m, y); }
+    warp_sums[lane] = m;
+  }
+  __syncthreads();
+  return max(wid ? warp_sums[wid - 1] : 0u, ex);
 }
 
 __global__ void __launch_bounds__(MERGE_THREADS, 3) k_merge_filter(MergeView V, const JobParams* prm, JobDev* J) {
@@ -695,15 +760,11 @@ __global__ void __launch_bounds__(MERGE_THREADS, 3) k_merge_filter(MergeView V, 
   unsigned long long* pfx2 = reinterpret_cast<unsigned long long*>(smem + L::A1 + L::PFX2_K * cap);
   uint8_t* recs = smem + L::A1 + L::RECS_K * cap;                   // cap * SS
   __shared__ uint32_t warp_sums[32];
-  __shared__ uint32_t sh_T, sh_ngroups, sh_any_filtered;
+  __shared__ uint32_t sh_T, sh_ngroups, sh_any_filtered, sh_any_id;
   __shared__ int sh_err;
   __shared__ uint32_t sh_c0;
-  __shared__ Overwrite sh_cot_ow[COT_MAX];       // table-level overwrite (slot 0) per distinct cotable id in the tile
-  __shared__ uint16_t sh_cot_li[COT_MAX];        // a record of the tile that carries the id bytes
-  __shared__ uint16_t sh_cot_len[COT_MAX];
-  __shared__ uint16_t sh_cand[COT_CAND_MAX];
-  __shared__ uint32_t sh_ncand;
-  __shared__ uint32_t sh_ncot;
+  __shared__ Overwrite sh_ow0;                   // slot 0 for the rows of the table the tile starts in, when looked up in the runs
+  __shared__ int sh_ow0_state;                   // 0 = not looked up, 1 = the rows start fresh, 2 = they start from sh_ow0
   __shared__ unsigned long long sh_stats[9];
   __shared__ const uint8_t* sh_pred;             // tile that starts inside a row group: the last visible record before it
   __shared__ uint32_t sh_rb[2][MAX_RUNS + 2];    // run boundaries of the merge tree (ping-pong per level)
@@ -733,6 +794,7 @@ __global__ void __launch_bounds__(MERGE_THREADS, 3) k_merge_filter(MergeView V, 
       seg_start[k] = acc;
       sh_T = acc;
       sh_any_filtered = 0;
+      sh_any_id = 0;
       sh_err = *reinterpret_cast<volatile int*>(&J->error);
     }
   }
@@ -886,6 +948,7 @@ __global__ void __launch_bounds__(MERGE_THREADS, 3) k_merge_filter(MergeView V, 
       if (V.fkh) V.fkh[gid] = (g < 0 || fk <= 0) ? 0u : leveldb_hash(e, static_cast<uint32_t>(fk), kBloomSeed);
     }
     if (rec_flags(e, S) & REC_F_INVISIBLE) sh_any_filtered = 1;
+    if (e[0] == 'y' || e[0] == '0') sh_any_id = 1;
   }
   __syncthreads();
   if (sh_err) return;                              // the job had failed already, or this tile's records are bad
@@ -982,97 +1045,52 @@ __global__ void __launch_bounds__(MERGE_THREADS, 3) k_merge_filter(MergeView V, 
     }
     rw_slot[i] = mark;
   }
-  if (threadIdx.x == 0) { sh_ncot = 0; sh_ncand = 0; }
-  __syncthreads();
-  // (d0) cotable / colocated tables: slot 0 of the overwrite stack (the table tombstone's time)
-  // carries over all rows of a table. The table-tombstone entries `id ! # HT` sort before every
-  // row of the table; they are looked up in the runs (binary search) and replayed, so that tiles
-  // stay independent. Only tiles that contain 'y' / '0' keys pay for this.
-  // Candidate groups (first row group of each id run) are found by all threads; thread 0 then
-  // replays the tombstones of the few distinct ids.
-  if (prm->R.enabled) {
-    for (uint32_t g = threadIdx.x; g < sh_ngroups; g += blockDim.x) {
-      const uint8_t* e = recs + static_cast<size_t>(SS) * order[gstart[g]];
-      const uint32_t ulen = rec_ulen(e, S);
-      if (ulen == 0 || (e[0] != 'y' && e[0] != '0')) continue;
-      const int id = dockey_id_size(e, ulen);
-      if (id <= 0 || static_cast<uint32_t>(id) >= ulen || e[id] == '!') continue;   // tombstone groups start fresh
-      if (g > 0) {
+  // (d0) cotable / colocated tables: slot 0 of the overwrite stack (the table tombstones' time) carries over all rows
+  // of a table. The tombstones `id ! # HT` sort before every row of their table, as one row group. The tile holds every
+  // entry between two splitters, so every id block of the tile (a maximal run of row groups with one id) other than the
+  // one the tile starts in also holds its table's tombstones, as its first group: a row group of such a table replays
+  // that group from shared memory. Only the block the tile starts in can have its tombstones in earlier tiles: thread 0
+  // replays them from the runs, once. Tiles stay independent, and tiles without 'y' / '0' keys skip all of this.
+  // After the scan, pvis[g] = the first group of the id block of group g (pvis is free once (c) is done).
+  const bool ids = prm->R.enabled && sh_any_id;
+  if (ids) {
+    const uint32_t ngroups = sh_ngroups;
+    if (threadIdx.x == 0) {
+      int state = 0;
+      const uint8_t* e = recs + static_cast<size_t>(SS) * order[0];
+      const uint32_t ul = rec_ulen(e, S);
+      const int id = table_id_len(e, ul);
+      if (id > 0 && static_cast<uint32_t>(id) < ul) {
+        bool lookup = e[id] != '!';                     // the tile starts among the table's rows
+        if (!lookup && cont && ngroups > 1) {           // it starts inside the tombstones: only rows of the table need them
+          const uint8_t* n1 = recs + static_cast<size_t>(SS) * order[gstart[1]];
+          lookup = rec_ulen(n1, S) > static_cast<uint32_t>(id) && n1[id] != '!' && common_prefix_len(n1, id, e, id) >= static_cast<uint32_t>(id);
+        }
+        if (lookup) {
+          const int rc = seed_table_from_runs(&sh_ow0, prm, V.runs, seg_lo, seg_start, k, S, e, id, e[id] == '!');
+          if (rc < 0) dev_fail(J, -rc, tile);
+          state = rc > 0 ? 2 : 1;
+        }
+      }
+      sh_ow0_state = state;
+    }
+    // mark every group that starts an id block (or has no id), then a max-scan carries the marks over the groups
+    const uint32_t per = (ngroups + blockDim.x - 1) / blockDim.x;
+    const uint32_t g0 = min(threadIdx.x * per, ngroups), g1 = min(g0 + per, ngroups);
+    uint32_t last = 0;                                  // 1 + the last mark in this thread's groups, 0 = none yet
+    for (uint32_t g = g0; g < g1; g++) {
+      bool head = g == 0;
+      if (!head) {
+        const uint8_t* e = recs + static_cast<size_t>(SS) * order[gstart[g]];
         const uint8_t* p = recs + static_cast<size_t>(SS) * order[gstart[g - 1]];
-        const uint32_t pl = rec_ulen(p, S);
-        if (pl > static_cast<uint32_t>(id) && p[id] != '!' && common_prefix_len(p, id, e, id) >= static_cast<uint32_t>(id)) continue;
+        const int id = table_id_len(e, rec_ulen(e, S));
+        head = id <= 0 || table_id_len(p, rec_ulen(p, S)) != id || common_prefix_len(p, id, e, id) < static_cast<uint32_t>(id);
       }
-      const uint32_t slot = atomicAdd(&sh_ncand, 1u);
-      if (slot < COT_CAND_MAX) sh_cand[slot] = static_cast<uint16_t>(g);
+      if (head) last = g + 1;
+      pvis[g] = static_cast<uint16_t>(last ? last - 1 : 0xffff);
     }
-  }
-  __syncthreads();
-  if (prm->R.enabled && threadIdx.x == 0 && sh_ncand) {
-    if (sh_ncand > COT_CAND_MAX) dev_fail(J, DEV_ERR_COTABLE, tile);
-    const uint32_t ncand = sh_ncand < COT_CAND_MAX ? sh_ncand : COT_CAND_MAX;
-    for (uint32_t q = 0; q < ncand; q++) {
-      const uint32_t g = sh_cand[q];
-      const uint32_t li = order[gstart[g]];
-      const uint8_t* e = recs + static_cast<size_t>(SS) * li;
-      const uint32_t ulen = rec_ulen(e, S);
-      const int id = dockey_id_size(e, ulen);
-      bool known = false;
-      for (uint32_t c = 0; c < sh_ncot && !known; c++) {
-        const uint8_t* o = recs + static_cast<size_t>(SS) * sh_cot_li[c];
-        known = (sh_cot_len[c] & 0x7fff) == id && common_prefix_len(o, id, e, id) >= static_cast<uint32_t>(id);
-      }
-      if (known) continue;
-      if (sh_ncot >= COT_MAX) { dev_fail(J, DEV_ERR_COTABLE, tile); break; }
-      // collect the table-tombstone entries of this id from all runs
-      const uint8_t* tomb[COT_TOMB_MAX]; int tomb_run[COT_TOMB_MAX]; uint32_t tomb_idx[COT_TOMB_MAX]; int nt = 0;
-      __align__(8) uint8_t pfxkey[24];
-      for (int q = 0; q < 24; q++) pfxkey[q] = q < id ? e[q] : (q == id ? '!' : 0);
-      bool overflow = false;
-      for (int r = 0; r < k && !overflow; r++) {
-        const RunView& run = V.runs[r];
-        uint32_t lo = 0, hi = run.n_entries;
-        while (lo < hi) {
-          const uint32_t mid = (lo + hi) >> 1;
-          const uint8_t* c = run.rec + static_cast<size_t>(mid) * S;
-          if (cmp_prefix_vs_key(pfxkey, id + 1, c, rec_ulen(c, S)) > 0) lo = mid + 1; else hi = mid;
-        }
-        for (uint32_t x = lo; x < run.n_entries; x++) {
-          const uint8_t* c = run.rec + static_cast<size_t>(x) * S;
-          const uint32_t cl = rec_ulen(c, S);
-          if (cl < static_cast<uint32_t>(id) + 1 || common_prefix_len(c, id + 1, pfxkey, id + 1) < static_cast<uint32_t>(id) + 1) break;
-          if (rec_flags(c, S) & REC_F_HT_FILTERED) continue;     // out-of-range tombstones DO seed the table state
-          if (nt >= COT_TOMB_MAX) { overflow = true; break; }
-          tomb[nt] = c; tomb_run[nt] = r; tomb_idx[nt] = x; nt++;
-        }
-      }
-      if (overflow) { dev_fail(J, DEV_ERR_COTABLE, tile); break; }
-      for (int a = 1; a < nt; a++)                      // insertion sort by internal key
-        for (int b = a; b > 0 && cmp_records(tomb[b], tomb[b - 1], S) < 0; b--) {
-          const uint8_t* tp = tomb[b]; tomb[b] = tomb[b - 1]; tomb[b - 1] = tp;
-          int tr = tomb_run[b]; tomb_run[b] = tomb_run[b - 1]; tomb_run[b - 1] = tr;
-          uint32_t ti = tomb_idx[b]; tomb_idx[b] = tomb_idx[b - 1]; tomb_idx[b - 1] = ti;
-        }
-      FeedState st;
-      feed_state_reset(&st);
-      for (int a = 0; a < nt; a++) {
-        const uint8_t* c = tomb[a];
-        if (a > 0 && cmp_user_keys(tomb[a - 1], rec_ulen(tomb[a - 1], S), c, rec_ulen(c, S)) == 0) continue;   // rule A
-        const uint64_t suffix = rec_suffix(c, S);
-        if ((suffix & 0xff) == 0 && prm->bottommost && (suffix >> 8) <= prm->last_sequence) continue;          // obsolete deletion
-        const uint32_t vlen = rec_vlen(c, S);
-        const uint8_t vfirst = rec_vfirst(c, S);
-        const uint8_t* val = nullptr;
-        if (vlen && has_control_fields(vfirst)) val = V.runs[tomb_run[a]].data + V.runs[tomb_run[a]].val_off[tomb_idx[a]];
-        ValueRewrite rw;
-        int d = feed_step(&st, prm->R, c, rec_ulen(c, S), vfirst, val, vlen, &rw);
-        if (d < 0) { dev_fail(J, -d, tile); break; }
-      }
-      const uint32_t c = sh_ncot;
-      sh_cot_li[c] = static_cast<uint16_t>(li); sh_cot_len[c] = static_cast<uint16_t>(id);
-      if (st.n_ow >= 1 && st.n_ends == 1) sh_cot_ow[c] = st.ow[0];
-      else { sh_cot_ow[c].ht = prm->R.ht_min_enc; sh_cot_ow[c].exp.ttl_ns = kMaxTtlNs; sh_cot_ow[c].exp.write_ht = 0; sh_cot_len[c] = static_cast<uint16_t>(0x8000 | id); }
-      sh_ncot = c + 1;
-    }
+    const uint32_t carry = block_exclusive_max(last, warp_sums);
+    for (uint32_t g = g0; g < g1 && pvis[g] == 0xffff; g++) pvis[g] = static_cast<uint16_t>(carry - 1);
   }
   __syncthreads();
   if (prm->R.enabled) {
@@ -1080,20 +1098,17 @@ __global__ void __launch_bounds__(MERGE_THREADS, 3) k_merge_filter(MergeView V, 
       FeedState st;
       feed_state_reset(&st);
       const uint32_t i0 = gstart[g], i1 = gstart[g + 1];
-      if (sh_ncot) {
+      if (ids) {
         const uint8_t* e0 = recs + static_cast<size_t>(SS) * order[i0];
         const uint32_t ul0 = rec_ulen(e0, S);
-        if (ul0 && (e0[0] == 'y' || e0[0] == '0')) {
-          const int id = dockey_id_size(e0, ul0);
-          if (id > 0 && static_cast<uint32_t>(id) < ul0 && e0[id] != '!') {
-            for (uint32_t c = 0; c < sh_ncot; c++) {
-              const uint32_t clen = sh_cot_len[c] & 0x7fff;
-              const uint8_t* o = recs + static_cast<size_t>(SS) * sh_cot_li[c];
-              if (clen == static_cast<uint32_t>(id) && common_prefix_len(o, id, e0, id) >= static_cast<uint32_t>(id)) {
-                if (!(sh_cot_len[c] & 0x8000)) feed_state_seed(&st, e0, id, sh_cot_ow[c]);   // 0x8000: no tombstones => fresh
-                break;
-              }
-            }
+        const int id = table_id_len(e0, ul0);
+        if (id > 0 && static_cast<uint32_t>(id) < ul0 && e0[id] != '!') {          // a row of a cotable / colocated table
+          const uint32_t h = pvis[g];
+          if (h == 0 && sh_ow0_state) {
+            if (sh_ow0_state == 2) feed_state_seed(&st, e0, id, sh_ow0);
+          } else if (recs[static_cast<size_t>(SS) * order[gstart[h]] + id] == '!') {   // the block starts with the tombstones
+            const int rc = seed_table_in_tile(&st, prm, V.runs, recs, SS, S, order, seg_lo, seg_start, gstart[h], gstart[h + 1], e0, id);
+            if (rc < 0) { dev_fail(J, -rc, tile); continue; }
           }
         }
       }
@@ -1436,7 +1451,6 @@ static const char* DevErrorName(int e) {
     case DEV_ERR_STACK_DEPTH: return "too many subkey levels";
     case DEV_ERR_UNSUPPORTED_VALUE: return "record type needs a host callback (packed row / merge / single delete)";
     case DEV_ERR_BAD_CRC: return "block checksum mismatch";
-    case DEV_ERR_COTABLE: return "cotable/colocated keys are not supported yet";
     case DEV_ERR_SHORT_KEY: return "internal key shorter than 8 bytes";
     case DEV_ERR_UNSORTED: return "input file is not sorted";
     default: return "unknown device error";
@@ -1446,7 +1460,7 @@ static const char* DevErrorName(int e) {
 static ybgpu_status DevErrorStatus(int e) {
   switch (e) {
     case DEV_ERR_COMPRESSED: case DEV_ERR_UNSUPPORTED_KEY: case DEV_ERR_UNSUPPORTED_VALUE:
-    case DEV_ERR_TILE_OVERFLOW: case DEV_ERR_COTABLE: case DEV_ERR_KEY_TOO_LONG: case DEV_ERR_STACK_DEPTH:
+    case DEV_ERR_TILE_OVERFLOW: case DEV_ERR_KEY_TOO_LONG: case DEV_ERR_STACK_DEPTH:
     case DEV_ERR_IRREGULAR_RESTARTS:
       return YBGPU_NOT_SUPPORTED;
     default: return YBGPU_CORRUPTION;
