@@ -188,7 +188,10 @@ enum {
   YBGPU_PATH_KV_INPUT = 64,            /* the inputs were KV streams (ybgpu_job_add_input_kv), not table files */
   YBGPU_PATH_SNAPPY_OUTPUT = 128,      /* output data blocks went through the GPU Snappy encoder (k_snappy_compress) */
   YBGPU_PATH_LZ4 = 256,                /* LZ4 (or LZ4HC) input blocks were uncompressed on the GPU */
-  YBGPU_PATH_LZ4_OUTPUT = 512          /* output data blocks went through the GPU LZ4 encoder (k_lz4_compress) */
+  YBGPU_PATH_LZ4_OUTPUT = 512,         /* output data blocks went through the GPU LZ4 encoder (k_lz4_compress) */
+  YBGPU_PATH_INGEST_RETRY = 1024,      /* k_ingest ran a second time at its widest record stride (a key longer than the probe's sample) */
+  YBGPU_PATH_FAST_DECODE = 2048,       /* the general path decoded with k_decode_fast<...> rather than k_decode_all<...> */
+  YBGPU_PATH_ENCODER_FUSED = 4096      /* k_encode_fused wrote the output blocks larger than k_encode_v4's shared-memory image */
 };
 
 typedef struct ybgpu_job ybgpu_job;

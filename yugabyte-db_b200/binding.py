@@ -78,6 +78,7 @@ PHASE_NAMES = ["block_scan", "decode", "partition", "merge_filter", "encode"]
 PATH_FUSED_INGEST, PATH_GENERAL_DECODE, PATH_SNAPPY, PATH_PARTITION_RETRY, PATH_ENCODER_V4, PATH_ENCODER_V5, PATH_KV_INPUT = 1, 2, 4, 8, 16, 32, 64
 PATH_SNAPPY_OUTPUT = 128
 PATH_LZ4, PATH_LZ4_OUTPUT = 256, 512
+PATH_INGEST_RETRY, PATH_FAST_DECODE, PATH_ENCODER_FUSED = 1024, 2048, 4096
 COMPRESSION_NONE, COMPRESSION_SNAPPY, COMPRESSION_LZ4 = 0, 1, 4   # output_compression (rocksdb::CompressionType)
 
 

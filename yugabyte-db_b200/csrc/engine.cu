@@ -2148,6 +2148,7 @@ ybgpu_status Engine::Run(const volatile int32_t* shutting_down) {
       if (ybgpu_status s = CheckDeviceError("ingest")) return s;
       if (I.hJ.ingest_fallback != ING_FALLBACK_WIDER || Sfinal == S_widest) break;
       Sfinal = S_widest;
+      stats_.path_flags |= YBGPU_PATH_INGEST_RETRY;
     }
     CUDA_TRY(end_phase());
     tick("ingest");
@@ -2223,6 +2224,7 @@ ybgpu_status Engine::Run(const volatile int32_t* shutting_down) {
       bool fast = d_range == nullptr && max_ikey <= 64;
       for (int r = 0; r < k; r++) fast = fast && I.runs[r].key_encoding == 1 && I.runs[r].ht_filter == 0xfffffffffffffffeull && I.runs[r].cf_n == 0;
       if (fast && getenv("YBGPU_NO_FAST_DECODE") == nullptr) {
+        stats_.path_flags |= YBGPU_PATH_FAST_DECODE;
         if (max_ikey <= 32) k_decode_fast<2><<<grid, 128, 0, I.stream>>>(I.dRuns, d_group_base, k, Sfinal, I.dJ);
         else if (max_ikey <= 48) k_decode_fast<3><<<grid, 128, 0, I.stream>>>(I.dRuns, d_group_base, k, Sfinal, I.dJ);
         else k_decode_fast<4><<<grid, 128, 0, I.stream>>>(I.dRuns, d_group_base, k, Sfinal, I.dJ);
@@ -2511,6 +2513,7 @@ ybgpu_status Engine::Run(const volatile int32_t* shutting_down) {
         if (total_and_max[1] > ENC_SMEM_CAP) {
           fused_kernel<<<std::min<uint32_t>(nblocks, sms * 4), ENC_THREADS, 0, I.stream>>>(E, Sfinal, I.d_block_first, nblocks, I.d_block_off, I.out_file, ENC_SMEM_CAP);
           launches++;
+          stats_.path_flags |= YBGPU_PATH_ENCODER_FUSED;
         }
       }
       CUDA_TRY(cudaEventRecord(I.enc_ev[1], I.stream));
