@@ -191,7 +191,8 @@ enum {
   YBGPU_PATH_LZ4_OUTPUT = 512,         /* output data blocks went through the GPU LZ4 encoder (k_lz4_compress) */
   YBGPU_PATH_INGEST_RETRY = 1024,      /* k_ingest ran a second time at its widest record stride (a key longer than the probe's sample) */
   YBGPU_PATH_FAST_DECODE = 2048,       /* the general path decoded with k_decode_fast<...> rather than k_decode_all<...> */
-  YBGPU_PATH_ENCODER_FUSED = 4096      /* k_encode_fused wrote the output blocks larger than k_encode_v4's shared-memory image */
+  YBGPU_PATH_ENCODER_FUSED = 4096,     /* k_encode_fused wrote the output blocks larger than k_encode_v4's shared-memory image */
+  YBGPU_PATH_OUTPUT_VERIFIED = 8192    /* ybgpu_job_verify_output re-read the finished table on the GPU and found it good */
 };
 
 typedef struct ybgpu_job ybgpu_job;
@@ -368,6 +369,22 @@ ybgpu_status ybgpu_compact_files_one_table(const ybgpu_job_options* options, con
                                            const volatile int32_t* shutting_down, ybgpu_one_table_result* result,
                                            ybgpu_job_stats* total, char* err, uint64_t err_cap);
 
+/* ybgpu_compact_files / ybgpu_compact_files_one_table with DBOptions::paranoid_file_checks: verify_outputs != 0 runs
+ * ybgpu_job_verify_output on every range, on the range's own stream, right after it ran and before its device->host copy
+ * starts, so a bad range fails the compaction before a byte of it reaches the caller's buffers (err: the first failing
+ * range's message). Every verified range carries YBGPU_PATH_OUTPUT_VERIFIED in its stats. verify_outputs == 0: exactly
+ * the unchecked calls. */
+ybgpu_status ybgpu_compact_files_checked(const ybgpu_job_options* options, const ybgpu_input_file* files, uint32_t num_files,
+                                         uint32_t max_subcompactions, uint32_t max_in_flight,
+                                         uint8_t* data_arena, uint64_t data_arena_cap, uint8_t* meta_arena, uint64_t meta_arena_cap,
+                                         const volatile int32_t* shutting_down, ybgpu_sub_output* outputs, uint32_t* num_outputs,
+                                         ybgpu_job_stats* total, char* err, uint64_t err_cap, int32_t verify_outputs);
+ybgpu_status ybgpu_compact_files_one_table_checked(const ybgpu_job_options* options, const ybgpu_input_file* files, uint32_t num_files,
+                                                   uint32_t max_subcompactions, uint32_t max_in_flight,
+                                                   uint8_t* data_out, uint64_t data_cap, uint8_t* meta_out, uint64_t meta_cap,
+                                                   const volatile int32_t* shutting_down, ybgpu_one_table_result* result,
+                                                   ybgpu_job_stats* total, char* err, uint64_t err_cap, int32_t verify_outputs);
+
 /* --- one oversized compaction, key-range sharded across the GPUs of a box (SURVEY.md 8e; BASELINE config 5) ----------
  * Replaces, across devices, what CompactionJob::GenSubcompactionBoundaries + the subcompaction threads do inside one
  * process (rocksdb/db/compaction_job.cc:409-519,532-552). One process per GPU; every rank holds some of the tablet's
@@ -424,6 +441,56 @@ ybgpu_status ybgpu_sst_concat_meta(const ybgpu_job_options* table_options, const
  * oracle. *bad_blocks > 0 => YBGPU_CORRUPTION. */
 ybgpu_status ybgpu_sst_verify_blocks(const uint8_t* meta_file, uint64_t meta_file_len, const uint8_t* data_file,
                                      uint64_t data_file_len, uint32_t stride, uint64_t* blocks_checked, uint64_t* bad_blocks);
+
+/* --- output check on the GPU ---------------------------------------------------------------------
+ * Replaces: CompactionJob::CheckOutputFile under DBOptions::paranoid_file_checks (compaction_job.cc:932-971), which
+ * re-opens the new table and iterates all of it. Here the finished data file is re-read while it is still in device
+ * memory, before any byte of it is copied to the host: the block assembler derives the trailers from checksums of the
+ * INPUT values and never reads a block back, so a trailer protects the reader but does not check the writer.
+ *   1. every block's masked CRC32C is recomputed from the stored bytes and compared with its trailer;
+ *   2. blocks stored compressed (Snappy, LZ4) are uncompressed into a scratch image; the stream must be well formed
+ *      and as long as its preamble says;
+ *   3. every entry is parsed the way BlockIter does (either key encoding): restart array inside the block, restart
+ *      offsets ascending and at entries that share nothing, every header and every entry inside the block;
+ *   4. internal keys strictly ascend inside every block and from block to block;
+ *   5. (jobs only) the table holds the merge result: per-block and total entry counts, the first / last key against
+ *      the boundary records of ybgpu_job_output_boundaries, and entry i of the table against survivor i — key bytes,
+ *      value length and value bytes, the latter read from where the merge left them (the input file, the re-encoded
+ *      control-field prefix, or "X" for a value that expired into a tombstone), not from the output.
+ * The first failure is the one with the lowest (block, entry), whatever the kernels' scheduling. */
+enum {
+  YBGPU_CHECK_OK = 0,
+  YBGPU_CHECK_CHECKSUM = 1,            /* stored bytes disagree with the block trailer */
+  YBGPU_CHECK_COMPRESSED_STREAM = 2,   /* a compressed block does not decode to the length it announces */
+  YBGPU_CHECK_ENTRY_PARSE = 3,         /* restart array or an entry header / body outside its block */
+  YBGPU_CHECK_KEY_ORDER = 4,           /* a key is not above its predecessor */
+  YBGPU_CHECK_ENTRY_COUNT = 5,         /* a block or the table holds another number of entries than the merge kept */
+  YBGPU_CHECK_CONTENTS = 6,            /* an entry's key or value differs from the survivor that belongs there */
+  YBGPU_CHECK_KEY_TOO_LONG = 7         /* ybgpu_sst_verify_device only: an internal key above 1016 bytes (NotSupported) */
+};
+typedef struct ybgpu_output_check {
+  uint64_t blocks_checked;             /* data blocks of the table */
+  uint64_t blocks_compressed;          /* ... of which stored compressed (trailer type != kNoCompression) */
+  uint64_t entries_parsed;
+  uint64_t bytes_read;                 /* stored table bytes + uncompressed bytes parsed (+ the values compared with, for a job) */
+  double gpu_seconds;                  /* device time of the check (CUDA events on the job's stream) */
+  uint32_t failure_kind;               /* YBGPU_CHECK_* of the first failure */
+  uint32_t failure_block;              /* its data block (index order) */
+  uint32_t failure_entry;              /* its entry inside that block (0 for failures of the block as a whole) */
+  uint32_t reserved;
+} ybgpu_output_check;
+
+/* Checks 1-5 on the output of a job. Legal after a successful ybgpu_job_run (YBGPU_ILLEGAL_STATE otherwise), any number
+ * of times, before or after the fetch calls. An empty output is YBGPU_OK with zero counts (compaction_job.cc:950-952).
+ * A failure returns YBGPU_CORRUPTION, fills *result and ybgpu_job_error; success sets YBGPU_PATH_OUTPUT_VERIFIED in the
+ * job's path_flags. The only large temporary is the uncompressed image of a compressed output; it is freed on return. */
+ybgpu_status ybgpu_job_verify_output(ybgpu_job* job, ybgpu_output_check* result);
+
+/* Checks 1-4 on ANY split SST held in host memory — the device counterpart of ybgpu_sst_verify_blocks, for a caller
+ * that wants to scrub an input or re-check a file it wrote. The data file is uploaded (32 MB chunks), checked and
+ * dropped. YBGPU_CORRUPTION with *result filled and the message in ybgpu_last_error on a failure. */
+ybgpu_status ybgpu_sst_verify_device(int32_t device, const uint8_t* meta_file, uint64_t meta_file_len,
+                                     const uint8_t* data_file, uint64_t data_file_len, ybgpu_output_check* result);
 
 /* Last internal key of a split SST (its last data block is decoded on the host): what
  * FileMetaData::largest holds for the file. key must hold 1032 bytes. */

@@ -79,7 +79,31 @@ PATH_FUSED_INGEST, PATH_GENERAL_DECODE, PATH_SNAPPY, PATH_PARTITION_RETRY, PATH_
 PATH_SNAPPY_OUTPUT = 128
 PATH_LZ4, PATH_LZ4_OUTPUT = 256, 512
 PATH_INGEST_RETRY, PATH_FAST_DECODE, PATH_ENCODER_FUSED = 1024, 2048, 4096
+PATH_OUTPUT_VERIFIED = 8192
 COMPRESSION_NONE, COMPRESSION_SNAPPY, COMPRESSION_LZ4 = 0, 1, 4   # output_compression (rocksdb::CompressionType)
+
+
+CHECK_KIND_NAMES = {0: "ok", 1: "checksum", 2: "compressed_stream", 3: "entry_parse", 4: "key_order", 5: "entry_count",
+                    6: "contents", 7: "key_too_long"}
+
+
+class OutputCheck(C.Structure):
+    """ybgpu_output_check: what the device-side table check read and, if it failed, where."""
+    _fields_ = [("blocks_checked", C.c_uint64), ("blocks_compressed", C.c_uint64), ("entries_parsed", C.c_uint64),
+                ("bytes_read", C.c_uint64), ("gpu_seconds", C.c_double), ("failure_kind", C.c_uint32),
+                ("failure_block", C.c_uint32), ("failure_entry", C.c_uint32), ("reserved", C.c_uint32)]
+
+    @property
+    def failure(self):
+        return CHECK_KIND_NAMES.get(self.failure_kind, str(self.failure_kind))
+
+
+class OutputCheckError(YbGpuError):
+    """A failed table check: .check is the OutputCheck with the first failure."""
+
+    def __init__(self, status, msg, check):
+        super().__init__(status, msg)
+        self.check = check
 
 
 class GenConfig(C.Structure):
@@ -361,6 +385,17 @@ class GpuCompactionJob:
         return ({a[i].tag: bytes(a[i].value[:a[i].len]) for i in range(n.value)},
                 {b[i].tag: bytes(b[i].value[:b[i].len]) for i in range(n.value)})
 
+    def verify_output(self):
+        """ybgpu_job_verify_output: re-reads the finished table on the GPU (checksums, compressed streams, every entry,
+        key order, contents against the merge result). Returns the OutputCheck; raises OutputCheckError on a failure."""
+        L = lib()
+        L.ybgpu_job_verify_output.argtypes = [C.c_void_p, C.POINTER(OutputCheck)]
+        chk = OutputCheck()
+        st = L.ybgpu_job_verify_output(self.h, C.byref(chk))
+        if st != 0:
+            raise OutputCheckError(st, L.ybgpu_job_error(self.h).decode(), chk)
+        return chk
+
     def digest(self):
         d = C.c_uint64()
         self._check(lib().ybgpu_job_kv_stream_digest(self.h, C.byref(d)))
@@ -603,13 +638,16 @@ class SubcompactionResult:
                 for o in self.outputs if o.data_len]
 
 
-def compact_files(ssts, max_subcompactions=8, max_in_flight=3, data_arena=None, meta_arena=None, ht_filters=None, cotable_filters=None, **job_kwargs):
+def compact_files(ssts, max_subcompactions=8, max_in_flight=3, data_arena=None, meta_arena=None, ht_filters=None, cotable_filters=None,
+                  verify_outputs=None, **job_kwargs):
     """ybgpu_compact_files: one compaction as pipelined key-range subcompactions (one output SST per
-    range, in range order). ssts: list of (meta ndarray, data ndarray) in host memory."""
+    range, in range order). ssts: list of (meta ndarray, data ndarray) in host memory. verify_outputs (True / False):
+    ybgpu_compact_files_checked, every range's table checked on the GPU before it is copied out."""
     L = lib()
     L.ybgpu_compact_files.argtypes = [C.POINTER(JobOptions), C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint64,
                                       C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.POINTER(C.c_uint32), C.POINTER(JobStats),
                                       C.c_char_p, C.c_uint64]
+    L.ybgpu_compact_files_checked.argtypes = L.ybgpu_compact_files.argtypes + [C.c_int32]
     o, keep_o = make_options(**job_kwargs)
     arr, keep = _input_files(ssts, ht_filters, cotable_filters)
     in_bytes = sum(int(d.size) for _, d in ssts)
@@ -621,8 +659,9 @@ def compact_files(ssts, max_subcompactions=8, max_in_flight=3, data_arena=None, 
     n = C.c_uint32()
     total = JobStats()
     err = C.create_string_buffer(512)
-    st = L.ybgpu_compact_files(C.byref(o), arr, len(ssts), max_subcompactions, max_in_flight, data_arena.ctypes.data, data_arena.size,
-                               meta_arena.ctypes.data, meta_arena.size, None, outs, C.byref(n), C.byref(total), err, 512)
+    args = (C.byref(o), arr, len(ssts), max_subcompactions, max_in_flight, data_arena.ctypes.data, data_arena.size,
+            meta_arena.ctypes.data, meta_arena.size, None, outs, C.byref(n), C.byref(total), err, 512)
+    st = L.ybgpu_compact_files(*args) if verify_outputs is None else L.ybgpu_compact_files_checked(*args, int(bool(verify_outputs)))
     if st != 0:
         raise YbGpuError(st, err.value.decode(errors="replace"))
     return SubcompactionResult([outs[i] for i in range(n.value)], total, data_arena, meta_arena)
@@ -642,13 +681,16 @@ class OneTableResult(C.Structure):
         return bytes(self.largest_key[:self.largest_key_len])
 
 
-def compact_files_one_table(ssts, max_subcompactions=8, max_in_flight=3, data_out=None, meta_out=None, ht_filters=None, cotable_filters=None, **job_kwargs):
+def compact_files_one_table(ssts, max_subcompactions=8, max_in_flight=3, data_out=None, meta_out=None, ht_filters=None, cotable_filters=None,
+                            verify_outputs=None, **job_kwargs):
     """ybgpu_compact_files_one_table: the pipelined compaction with ONE output table. Returns
-    (data view, meta view, OneTableResult, total JobStats)."""
+    (data view, meta view, OneTableResult, total JobStats). verify_outputs (True / False):
+    ybgpu_compact_files_one_table_checked, every range checked on the GPU before it is copied out."""
     L = lib()
     L.ybgpu_compact_files_one_table.argtypes = [C.POINTER(JobOptions), C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint64,
                                                 C.c_void_p, C.c_uint64, C.c_void_p, C.POINTER(OneTableResult), C.POINTER(JobStats),
                                                 C.c_char_p, C.c_uint64]
+    L.ybgpu_compact_files_one_table_checked.argtypes = L.ybgpu_compact_files_one_table.argtypes + [C.c_int32]
     o, keep_o = make_options(**job_kwargs)
     arr, keep = _input_files(ssts, ht_filters, cotable_filters)
     in_bytes = sum(int(d.size) for _, d in ssts)
@@ -659,8 +701,9 @@ def compact_files_one_table(ssts, max_subcompactions=8, max_in_flight=3, data_ou
     res = OneTableResult()
     total = JobStats()
     err = C.create_string_buffer(512)
-    st = L.ybgpu_compact_files_one_table(C.byref(o), arr, len(ssts), max_subcompactions, max_in_flight, data_out.ctypes.data, data_out.size,
-                                         meta_out.ctypes.data, meta_out.size, None, C.byref(res), C.byref(total), err, 512)
+    args = (C.byref(o), arr, len(ssts), max_subcompactions, max_in_flight, data_out.ctypes.data, data_out.size,
+            meta_out.ctypes.data, meta_out.size, None, C.byref(res), C.byref(total), err, 512)
+    st = L.ybgpu_compact_files_one_table(*args) if verify_outputs is None else L.ybgpu_compact_files_one_table_checked(*args, int(bool(verify_outputs)))
     if st != 0:
         raise YbGpuError(st, err.value.decode(errors="replace"))
     return data_out[:res.data_len], meta_out[:res.meta_len], res, total
@@ -795,3 +838,17 @@ def sst_verify_blocks(meta, data, stride=1):
     if st not in (0, 2):
         raise YbGpuError(st, L.ybgpu_last_error().decode())
     return n.value, bad.value
+
+
+def sst_verify_device(meta, data, device=0):
+    """ybgpu_sst_verify_device: checksums, compressed streams, every entry and the key order of a split SST, checked on
+    the GPU. Returns the OutputCheck; raises OutputCheckError (Corruption, .check = the first failure) for a bad table."""
+    L = lib()
+    L.ybgpu_sst_verify_device.argtypes = [C.c_int32, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64, C.POINTER(OutputCheck)]
+    meta = np.ascontiguousarray(np.frombuffer(meta, np.uint8) if isinstance(meta, (bytes, bytearray)) else meta, dtype=np.uint8)
+    data = np.ascontiguousarray(np.frombuffer(data, np.uint8) if isinstance(data, (bytes, bytearray)) else data, dtype=np.uint8)
+    chk = OutputCheck()
+    st = L.ybgpu_sst_verify_device(device, meta.ctypes.data, meta.size, data.ctypes.data if data.size else None, data.size, C.byref(chk))
+    if st != 0:
+        raise OutputCheckError(st, L.ybgpu_last_error().decode(), chk)
+    return chk

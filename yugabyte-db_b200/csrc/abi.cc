@@ -130,6 +130,30 @@ ybgpu_status ybgpu_job_run(ybgpu_job* job, const volatile int32_t* shutting_down
   return Sync(job, job->engine->Run(shutting_down));
 }
 
+ybgpu_status ybgpu_job_verify_output(ybgpu_job* job, ybgpu_output_check* result) {
+  if (!job || !result) return YBGPU_INVALID_ARGUMENT;
+  return Sync(job, job->engine->VerifyOutput(result));
+}
+
+ybgpu_status ybgpu_sst_verify_device(int32_t device, const uint8_t* meta, uint64_t meta_len, const uint8_t* data, uint64_t data_len,
+                                     ybgpu_output_check* result) {
+  if (!meta || (!data && data_len) || !result) { g_last_error = "null argument"; return YBGPU_INVALID_ARGUMENT; }
+  ybgpu::host::SstMeta m;
+  std::string err = ybgpu::host::ParseSplitSstMeta(meta, meta_len, &m);
+  if (!err.empty()) { g_last_error = err; return YBGPU_CORRUPTION; }
+  std::vector<ybgpu_block_handle> h(m.data_blocks.size());
+  for (size_t i = 0; i < h.size(); i++) { h[i].offset = m.data_blocks[i].offset; h[i].size = m.data_blocks[i].size; }
+  ybgpu_job_options o;
+  ybgpu_job_options_init(&o);
+  o.device = device;
+  o.cuda_stream = YBGPU_STREAM_PRIVATE;
+  Engine e(o);
+  ybgpu_status s = e.Init();
+  if (s == YBGPU_OK) s = e.VerifySst(data, data_len, h.data(), h.size(), m.key_encoding, result);
+  if (s != YBGPU_OK) g_last_error = e.error();
+  return s;
+}
+
 ybgpu_status ybgpu_job_get_stats(const ybgpu_job* job, ybgpu_job_stats* stats) {
   if (!job || !stats) return YBGPU_INVALID_ARGUMENT;
   *stats = const_cast<ybgpu_job*>(job)->engine->stats();

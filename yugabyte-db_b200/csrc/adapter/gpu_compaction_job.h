@@ -321,6 +321,10 @@ class GpuCompactionJob {
     // (util/file_reader_writer.cc:343): called between kernel phases and between subcompaction ranges.
     void (*yield_fn)(void*) = nullptr;
     void* yield_ctx = nullptr;
+    // DBOptions::paranoid_file_checks (compaction_job.cc:932-971): Run() re-reads every finished table on the GPU before
+    // it is copied to the host (ybgpu_job_verify_output: checksums, compressed streams, every entry, key order, contents
+    // against the merge result) and returns Corruption instead of an output that fails it.
+    bool paranoid_file_checks = false;
   };
 
   explicit GpuCompactionJob(const Params& p) : p_(p) {}
@@ -381,6 +385,10 @@ class GpuCompactionJob {
     }
     ybgpu_status s = ybgpu_job_run(job_, p_.shutting_down);
     if (s != YBGPU_OK) return ToStatus(s, ybgpu_job_error(job_));
+    if (p_.paranoid_file_checks) {
+      s = ybgpu_job_verify_output(job_, &output_check_);
+      if (s != YBGPU_OK) return ToStatus(s, ybgpu_job_error(job_));
+    }
     uint64_t dl = 0, ml = 0;
     s = ybgpu_job_output_sizes(job_, &dl, &ml);
     if (s != YBGPU_OK) return ToStatus(s, ybgpu_job_error(job_));
@@ -421,10 +429,10 @@ class GpuCompactionJob {
     std::vector<ybgpu_sub_output> outs(p_.max_subcompactions);
     uint32_t n = 0;
     char err[512] = {0};
-    ybgpu_status s = ybgpu_compact_files(&o, files.data(), static_cast<uint32_t>(files.size()), p_.max_subcompactions,
-                                         p_.subcompactions_in_flight, reinterpret_cast<uint8_t*>(&data_arena[0]), data_arena.size(),
-                                         reinterpret_cast<uint8_t*>(&meta_arena[0]), meta_arena.size(), p_.shutting_down,
-                                         outs.data(), &n, &stats_, err, sizeof(err));
+    ybgpu_status s = ybgpu_compact_files_checked(&o, files.data(), static_cast<uint32_t>(files.size()), p_.max_subcompactions,
+                                                 p_.subcompactions_in_flight, reinterpret_cast<uint8_t*>(&data_arena[0]), data_arena.size(),
+                                                 reinterpret_cast<uint8_t*>(&meta_arena[0]), meta_arena.size(), p_.shutting_down,
+                                                 outs.data(), &n, &stats_, err, sizeof(err), p_.paranoid_file_checks ? 1 : 0);
     if (s != YBGPU_OK) return ToStatus(s, err);
     outputs_.clear();
     for (uint32_t i = 0; i < n; i++) {
@@ -442,6 +450,8 @@ class GpuCompactionJob {
     return Status::OK();
   }
   const std::vector<OutputFile>& outputs() const { return outputs_; }
+  // What the device check of Run() read (Params::paranoid_file_checks, single-output jobs); zeroes otherwise.
+  const ybgpu_output_check& output_check() const { return output_check_; }
   // Inputs that take part in the merge: all but the files marked delete_after_compaction (COMPACTION_FILES_NOT_FILTERED /
   // COMPACTION_FILES_FILTERED tickers, db/version_set.cc:3817-3820).
   size_t NumReadInputs() const { size_t n = 0; for (const InputFile& f : inputs_) n += !f.delete_after_compaction; return n; }
@@ -664,6 +674,7 @@ class GpuCompactionJob {
   std::vector<OutputFile> outputs_;
   ybgpu_job_options options_{};
   ybgpu_job_stats stats_{};
+  ybgpu_output_check output_check_{};
 };
 
 }  // namespace ybgpu_adapter

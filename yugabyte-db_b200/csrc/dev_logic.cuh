@@ -1214,4 +1214,126 @@ YB_HD_NOINLINE int replay_table_seed(FeedState* st, const RetentionDev& R, const
   return 0;
 }
 
+// ---- output check (V): what a reader finds in a finished data block ---------------------------------------------------
+// The judgement of the device-side table check (verify_kernels.cuh), shared with the CPU tests: the walk of one restart
+// interval the way BlockIter::ParseNextKey does it (table/block.cc:294-447), in either key encoding, with every key
+// rebuilt, compared with its predecessor in InternalKeyComparator order (db/dbformat.cc:92-114) and handed to `expect`
+// together with its value. Numbered like ybgpu_output_check::failure_kind.
+enum VerifyKind : uint32_t {
+  VERIFY_OK = 0, VERIFY_CHECKSUM = 1, VERIFY_COMPRESSED = 2, VERIFY_PARSE = 3, VERIFY_ORDER = 4, VERIFY_COUNT = 5,
+  VERIFY_CONTENTS = 6, VERIFY_KEY_TOO_LONG = 7,
+};
+constexpr uint32_t VERIFY_MAX_IKEY = 1008 + 8;         // the engine's key limit: longer keys are not rebuilt
+
+// First failure of a table: the lowest (block, entry) wins whatever the scheduling, so the three are packed into one word
+// for atomicMin. ~0 = no failure.
+YB_HD unsigned long long verify_pack(uint32_t block, uint32_t entry, uint32_t kind) {
+  return (static_cast<unsigned long long>(block) << 32) | (static_cast<unsigned long long>(entry < 0x0fffffffu ? entry : 0x0fffffffu) << 4) | kind;
+}
+
+YB_HD int cmp_internal_keys(const uint8_t* a, uint32_t la, const uint8_t* b, uint32_t lb) {
+  const int r = cmp_raw(a, la - 8, b, lb - 8);
+  if (r) return r;
+  uint64_t sa = 0, sb = 0;
+  for (int i = 7; i >= 0; i--) { sa = (sa << 8) | a[la - 8 + i]; sb = (sb << 8) | b[lb - 8 + i]; }
+  return sa > sb ? -1 : (sa < sb ? 1 : 0);
+}
+
+// The restart array of a block of `size` bytes (Block::Block / NumRestarts, table/block.cc:449-470): at least one restart
+// point, the array inside the block. A data block without entries is never written (BlockBasedTableBuilder::Flush).
+YB_HD bool verify_block_layout(const uint8_t* blk, uint32_t size, uint32_t* num_restarts, uint32_t* restarts_off) {
+  if (size < 8) return false;
+  const uint32_t nr = ld_u32_unaligned(blk + size - 4);
+  if (nr == 0 || static_cast<uint64_t>(nr) * 4 + 4 > size) return false;
+  *num_restarts = nr; *restarts_off = size - 4 - 4 * nr;
+  return *restarts_off > 0;
+}
+// [*p, *end) of restart interval r: offsets ascend, the first is 0, the last interval ends at the restart array.
+YB_HD bool verify_interval_bounds(const uint8_t* blk, uint32_t num_restarts, uint32_t restarts_off, uint32_t r, uint32_t* p, uint32_t* end) {
+  *p = ld_u32_unaligned(blk + restarts_off + 4 * r);
+  *end = r + 1 < num_restarts ? ld_u32_unaligned(blk + restarts_off + 4 * (r + 1)) : restarts_off;
+  return (r != 0 || *p == 0) && *p < *end && *end <= restarts_off;
+}
+
+// The key of the entry at a restart point: it shares nothing, so its bytes are in the block itself. false = no such entry.
+YB_HD bool verify_restart_key(const uint8_t* blk, uint32_t p, uint32_t end, int key_encoding, const uint8_t** key, uint32_t* klen) {
+  uint32_t h, kl, vl;
+  if (key_encoding == 2) {
+    TspHeader th;
+    h = static_cast<uint32_t>(parse_entry_header_tsp(blk + p, end - p, &th));
+    if (!h || th.something_shared) return false;
+    kl = th.ns1; vl = th.vlen;
+  } else {
+    uint32_t shared;
+    h = static_cast<uint32_t>(parse_entry_header(blk + p, end - p, &shared, &kl, &vl));
+    if (!h || shared) return false;
+  }
+  if (kl < 8 || static_cast<uint64_t>(p) + h + kl + vl > end) return false;
+  *key = blk + p + h; *klen = kl;
+  return true;
+}
+
+struct VerifyWalk {
+  uint32_t n;                  // entries parsed before the walk ended
+  uint32_t kind;               // VERIFY_OK or what stopped it, at entry n of the interval
+  const uint8_t* last_key;     // the last key parsed (inside one of the two key buffers) and its length
+  uint32_t last_klen;
+};
+struct VerifyNoExpect {        // a table with nothing to compare it with (ybgpu_sst_verify_device)
+  YB_HD bool operator()(uint32_t, const uint8_t*, uint32_t, const uint8_t*, uint32_t) const { return true; }
+};
+
+// Entries [p, end) of one restart interval. buf0 / buf1: two key buffers of `kcap` bytes; expect(ordinal, key, klen,
+// value, vlen) says whether entry `ordinal` = ord_base + position of the table is the one that belongs there. No byte
+// outside [blk + p, blk + end) is read, whatever the block holds.
+template <class Expect>
+YB_HD void verify_interval(const uint8_t* blk, uint32_t p, uint32_t end, int key_encoding, uint8_t* buf0, uint8_t* buf1,
+                                    uint32_t kcap, uint32_t ord_base, const Expect& expect, VerifyWalk* w) {
+  uint8_t* cur = buf0; uint8_t* prev = buf1;
+  uint32_t prev_klen = 0, n = 0, kind = VERIFY_OK;
+  while (p < end) {
+    uint32_t klen, vlen;
+    if (key_encoding == 2) {
+      TspHeader th; uint32_t ms, ml;
+      const int h = parse_entry_header_tsp(blk + p, end - p, &th);
+      if (!h || (n == 0 && th.something_shared) || !tsp_key_layout(th, prev_klen, &klen, &ms, &ml) ||
+          static_cast<uint64_t>(p) + h + th.ns1 + th.ns2 + th.vlen > end || klen < 8) { kind = VERIFY_PARSE; break; }
+      if (klen > kcap) { kind = VERIFY_KEY_TOO_LONG; break; }
+      p += h;
+      uint32_t o = 0;
+      if (!th.something_shared) {
+        for (; o < th.ns1; o++) cur[o] = blk[p + o];
+      } else {
+        uint64_t last = 0;
+        if (th.last_size) { for (int i = 7; i >= 0; i--) last = (last << 8) | prev[prev_klen - 8 + i]; last += th.last_inc; }
+        for (; o < th.shared_prefix; o++) cur[o] = prev[o];
+        for (uint32_t i = 0; i < th.ns1; i++) cur[o++] = blk[p + i];
+        for (uint32_t i = 0; i < ml; i++) cur[o++] = prev[ms + i];
+        for (uint32_t i = 0; i < th.ns2; i++) cur[o++] = blk[p + th.ns1 + i];
+        if (th.last_size) for (int i = 0; i < 8; i++) cur[o++] = static_cast<uint8_t>(last >> (8 * i));
+      }
+      p += th.ns1 + th.ns2;
+      vlen = th.vlen;
+    } else {
+      uint32_t shared, non_shared;
+      const int h = parse_entry_header(blk + p, end - p, &shared, &non_shared, &vlen);
+      if (!h || shared > prev_klen || (n == 0 && shared != 0) || static_cast<uint64_t>(p) + h + non_shared + vlen > end ||
+          shared + non_shared < 8) { kind = VERIFY_PARSE; break; }
+      klen = shared + non_shared;
+      if (klen > kcap) { kind = VERIFY_KEY_TOO_LONG; break; }
+      p += h;
+      for (uint32_t i = 0; i < shared; i++) cur[i] = prev[i];
+      for (uint32_t i = 0; i < non_shared; i++) cur[shared + i] = blk[p + i];
+      p += non_shared;
+    }
+    if (n > 0 && cmp_internal_keys(prev, prev_klen, cur, klen) >= 0) { kind = VERIFY_ORDER; break; }
+    if (!expect(ord_base + n, cur, klen, blk + p, vlen)) { kind = VERIFY_CONTENTS; break; }
+    p += vlen;
+    uint8_t* t = cur; cur = prev; prev = t;
+    prev_klen = klen;
+    n++;
+  }
+  w->n = n; w->kind = kind; w->last_key = prev; w->last_klen = prev_klen;
+}
+
 }  // namespace ybgpu

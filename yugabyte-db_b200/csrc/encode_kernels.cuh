@@ -683,7 +683,8 @@ __device__ uint32_t warp_crc32c_strided(const uint8_t* p, uint64_t len, int lane
   return ~r;
 }
 
-// mode 0: write trailers of freshly encoded blocks. mode 1: verify stored trailers (inputs).
+// mode 0: write trailers of freshly encoded blocks. mode 1: verify stored trailers (inputs). mode 2: verify the stored
+// trailers of a finished table for the output check, which reports the lowest failing block (JobDev::verify_fail).
 __global__ void __launch_bounds__(256) k_crc_blocks(uint8_t* file, const unsigned long long* off, const uint32_t* size32,
                                                     const unsigned long long* size_from_next, uint32_t nblocks, int mode, JobDev* J) {
   __shared__ uint32_t tab0[256];
@@ -704,7 +705,10 @@ __global__ void __launch_bounds__(256) k_crc_blocks(uint8_t* file, const unsigne
       if (lane < 4) p[len + 1 + lane] = static_cast<uint8_t>(crc >> (8 * lane));
     } else {
       const uint32_t stored = ldg_u32_unaligned(p + len + 1);
-      if (lane == 0 && stored != crc) dev_fail(J, DEV_ERR_BAD_CRC, b);
+      if (lane == 0 && stored != crc) {
+        if (mode == 2) atomicMin(&J->verify_fail, verify_pack(b, 0, VERIFY_CHECKSUM));
+        else dev_fail(J, DEV_ERR_BAD_CRC, b);
+      }
     }
   }
 }

@@ -72,6 +72,7 @@ struct JobDev {                 // device-global job state
   uint32_t n_lz4;               // ... of which LZ4 or LZ4HC
   uint32_t n_cont_tiles;        // merge tiles that started inside a row group
   unsigned long long digest;
+  unsigned long long verify_fail; // output check: verify_pack() of the first failure, lowest (block, entry) wins; ~0 = none
 };
 
 struct JobParams {
@@ -1431,6 +1432,7 @@ __global__ void __launch_bounds__(256) k_digest(const uint8_t* keys, const uint6
 #include "encode_kernels.cuh"
 #include "ingest_kernels.cuh"
 #include "snappy_kernels.cuh"   // and lz4_kernels.cuh
+#include "verify_kernels.cuh"
 namespace ybgpu {
 
 // =============================================================================================
@@ -1922,6 +1924,28 @@ ybgpu_status Engine::CheckDeviceError(const char* phase) {
   return YBGPU_OK;
 }
 
+// Per-device one-time state (SM count, CRC tables in device memory), shared by every job of the
+// process; jobs may run concurrently on different host threads, so it is built under a lock and
+// the table kernels are complete before any job proceeds.
+static cudaError_t EnsureDeviceTables(int device, cudaStream_t stream, int* sms) {
+  static std::mutex dev_init_mu;
+  static int sm_count[64] = {};
+  static bool crc_ready[64] = {};
+  std::lock_guard<std::mutex> lock(dev_init_mu);
+  cudaError_t e;
+  // cudaGetDeviceProperties costs milliseconds per call; one attribute, cached per device.
+  if (!sm_count[device & 63] && (e = cudaDeviceGetAttribute(&sm_count[device & 63], cudaDevAttrMultiProcessorCount, device)) != cudaSuccess) return e;
+  if (!crc_ready[device & 63]) {
+    k_crc_init<<<1, 256, 0, stream>>>();
+    k_crc_init_xpow<<<(CRC_XPOW_TABLE + 256) / 256, 256, 0, stream>>>();
+    if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    if ((e = cudaStreamSynchronize(stream)) != cudaSuccess) return e;
+    crc_ready[device & 63] = true;
+  }
+  *sms = sm_count[device & 63];
+  return cudaSuccess;
+}
+
 ybgpu_status Engine::Run(const volatile int32_t* shutting_down) {
   if (ran_) return Fail(YBGPU_ILLEGAL_STATE, "job already ran");
   Impl& I = *impl_;
@@ -1929,25 +1953,8 @@ ybgpu_status Engine::Run(const volatile int32_t* shutting_down) {
   auto t_prev = std::chrono::steady_clock::now();
   CUDA_TRY(cudaSetDevice(opt_.device));
   g_alloc_stream = I.stream;
-  // Per-device one-time state (SM count, CRC tables in device memory), shared by every job of the
-  // process; jobs may run concurrently on different host threads, so it is built under a lock and
-  // the table kernels are complete before any job proceeds.
-  static std::mutex dev_init_mu;
-  static int sm_count[64] = {};
-  static bool crc_ready[64] = {};
-  {
-    std::lock_guard<std::mutex> lock(dev_init_mu);
-    // cudaGetDeviceProperties costs milliseconds per call; one attribute, cached per device.
-    if (!sm_count[opt_.device & 63]) CUDA_TRY(cudaDeviceGetAttribute(&sm_count[opt_.device & 63], cudaDevAttrMultiProcessorCount, opt_.device));
-    if (!crc_ready[opt_.device & 63]) {
-      k_crc_init<<<1, 256, 0, I.stream>>>();
-      k_crc_init_xpow<<<(CRC_XPOW_TABLE + 256) / 256, 256, 0, I.stream>>>();
-      CUDA_TRY(cudaGetLastError());
-      CUDA_TRY(cudaStreamSynchronize(I.stream));
-      crc_ready[opt_.device & 63] = true;
-    }
-  }
-  const int sms = sm_count[opt_.device & 63];
+  int sms = 0;
+  CUDA_TRY(EnsureDeviceTables(opt_.device, I.stream, &sms));
   const int k = static_cast<int>(I.runs.size());
   // the yield point sits where the shutdown flag is polled: between kernel phases
   auto shutdown = [&]() {
@@ -2855,6 +2862,180 @@ ybgpu_status Engine::Digest(uint64_t* digest) {
   CUDA_TRY(cudaStreamSynchronize(I.stream));
   *digest = I.hJ.digest;
   return YBGPU_OK;
+}
+
+// =============================================================================================
+// V: output check (verify_kernels.cuh)
+// =============================================================================================
+namespace {
+// Temporaries of one check, from the stream-ordered pool; returned to it when the check ends, however it ends.
+struct VerifyScratch {
+  cudaStream_t stream;
+  std::vector<void*> ptrs;
+  explicit VerifyScratch(cudaStream_t s) : stream(s) {}
+  ~VerifyScratch() { for (void* p : ptrs) cudaFreeAsync(p, stream); }
+  template <typename T>
+  cudaError_t Alloc(T** out, size_t count) {
+    void* p = nullptr;
+    cudaError_t e = cudaMallocAsync(&p, std::max<size_t>(count * sizeof(T), 16) + 32, stream);
+    if (e == cudaSuccess) { ptrs.push_back(p); *out = reinterpret_cast<T*>(p); }
+    return e;
+  }
+};
+const char* VerifyKindName(uint32_t kind) {
+  switch (kind) {
+    case VERIFY_CHECKSUM: return "block checksum mismatch";
+    case VERIFY_COMPRESSED: return "compressed block does not decode";
+    case VERIFY_PARSE: return "entry does not parse";
+    case VERIFY_ORDER: return "keys out of order";
+    case VERIFY_COUNT: return "entry count differs from the merge result";
+    case VERIFY_CONTENTS: return "entry differs from the merge result";
+    case VERIFY_KEY_TOO_LONG: return "internal key longer than 1016 bytes";
+    default: return "unknown failure";
+  }
+}
+}  // namespace
+
+// The table at `file`: nb blocks at d_off (nb + 1 offsets back to back when d_size is null, else with the contents sizes
+// d_size). job: also against the merge result of this engine's run.
+ybgpu_status Engine::VerifyTable(const uint8_t* file, uint64_t file_len, const unsigned long long* d_off, const uint32_t* d_size,
+                                 uint32_t nb, int key_encoding, bool job, ybgpu_output_check* result) {
+  Impl& I = *impl_;
+  memset(result, 0, sizeof(*result));
+  if (nb == 0) return YBGPU_OK;                            // no table was written (compaction_job.cc:950-952)
+  int sms = 0;
+  CUDA_TRY(EnsureDeviceTables(opt_.device, I.stream, &sms));
+  VerifyScratch T(I.stream);
+  cudaEvent_t ev[2] = {};
+  for (auto& e : ev) CUDA_TRY(cudaEventCreate(&e));
+  struct EvGuard { cudaEvent_t* e; ~EvGuard() { cudaEventDestroy(e[0]); cudaEventDestroy(e[1]); } } ev_guard{ev};
+  JobDev* dV = nullptr;
+  uint32_t* d_sz = nullptr;
+  CUDA_TRY(T.Alloc(&dV, 1));
+  CUDA_TRY(T.Alloc(&d_sz, nb));
+  JobDev hV{}; hV.verify_fail = ~0ull;
+  CUDA_TRY(cudaEventRecord(ev[0], I.stream));
+  if (ybgpu_status us = UploadSmall(dV, &hV, sizeof(hV))) return us;
+  k_verify_sizes<<<GridFor(nb, 256, sms), 256, 0, I.stream>>>(file, d_off, d_size, nb, d_sz, dV);
+  k_crc_blocks<<<GridFor(static_cast<uint64_t>(nb) * 32, 256, sms), 256, 0, I.stream>>>(const_cast<uint8_t*>(file), d_off, d_sz, nullptr, nb, 2, dV);
+  CUDA_TRY(cudaGetLastError());
+  if (ybgpu_status s = ReadSmall(&hV, dV, sizeof(JobDev))) return s;
+  result->blocks_checked = nb;
+  result->blocks_compressed = hV.n_compressed;
+  result->bytes_read = file_len;
+
+  VerifyView V{};
+  V.data = file; V.off = d_off; V.size = d_sz; V.nblocks = nb; V.key_encoding = key_encoding;
+  if (hV.n_compressed) {
+    // ---- what ReadBlock would hand to BlockIter: one uncompressed image of the table (UncompressBlockContents,
+    // table/format.cc:441-500), by the kernels that uncompress input tables
+    RunView rv{};
+    rv.data = file; rv.blk_off = reinterpret_cast<const uint64_t*>(d_off); rv.blk_size = d_sz; rv.nb = nb;
+    const uint32_t base[2] = {0, nb};
+    RunView* d_run = nullptr; uint32_t* d_base = nullptr; unsigned long long* d_img = nullptr;
+    SnapView sv{};
+    CUDA_TRY(T.Alloc(&d_run, 1)); CUDA_TRY(T.Alloc(&d_base, 2)); CUDA_TRY(T.Alloc(&d_img, 1));
+    CUDA_TRY(T.Alloc(&sv.out_off, static_cast<size_t>(nb) + 1)); CUDA_TRY(T.Alloc(&sv.usize, nb));
+    if (ybgpu_status us = UploadSmall(d_run, &rv, sizeof(rv))) return us;
+    if (ybgpu_status us = UploadSmall(d_base, base, sizeof(base))) return us;
+    sv.runs = d_run; sv.blk_base = d_base; sv.k = 1;
+    k_snappy_sizes<<<GridFor(nb, 256, sms), 256, 0, I.stream>>>(sv, dV);
+    k_scan_u64_single<<<1, 1024, 0, I.stream>>>(sv.out_off, nb, d_img);
+    CUDA_TRY(cudaGetLastError());
+    unsigned long long img_bytes = 0;
+    if (ybgpu_status s = ReadSmall(&img_bytes, d_img, 8)) return s;
+    if (ybgpu_status s = ReadSmall(&hV, dV, sizeof(JobDev))) return s;
+    // no Snappy or LZ4 stream grows more than 255-fold: a larger announcement is a damaged preamble, not an image to allocate
+    if (!hV.error && img_bytes > 256 * file_len + 5ull * nb) { hV.error = DEV_ERR_BAD_BLOCK; hV.error_where = 0; }
+    if (!hV.error) {
+      uint8_t* img = nullptr;
+      CUDA_TRY(T.Alloc(&img, img_bytes + 96));
+      CUDA_TRY(cudaMemsetAsync(img, 0, 16, I.stream));
+      CUDA_TRY(cudaMemsetAsync(img + 16 + img_bytes, 0, 64, I.stream));
+      sv.out = img + 16;
+      k_snappy_decode<<<sms * 8, 128, 0, I.stream>>>(sv, dV);
+      CUDA_TRY(cudaGetLastError());
+      V.data = img + 16; V.off = sv.out_off; V.size = sv.usize;
+      result->bytes_read += img_bytes;
+    }
+  }
+  if (!hV.error) {
+    V.ri = job ? static_cast<uint32_t>(opt_.block_restart_interval) : 0u;
+    V.kcap = job ? I.boundary_stride : VERIFY_MAX_IKEY;
+    V.kstride = (V.kcap + 15u) & ~15u;
+    auto kern = job ? k_verify_blocks<true> : k_verify_blocks<false>;
+    int occ = 0;
+    CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, VERIFY_THREADS, 0));
+    // a persistent grid: as many warps as stay resident (fewer for a table that came from outside, whose key buffers are sized for the longest key)
+    const uint32_t per_sm = static_cast<uint32_t>(std::max(1, job ? occ : std::min(occ, 4)));
+    const uint32_t grid = std::min<uint32_t>((nb + VERIFY_THREADS / 32 - 1) / (VERIFY_THREADS / 32), static_cast<uint32_t>(sms) * per_sm);
+    CUDA_TRY(T.Alloc(&V.keybuf, static_cast<size_t>(grid) * VERIFY_THREADS * 2 * V.kstride));
+    if (job) { V.block_first = I.d_block_first; V.boundary = I.d_boundary; V.boundary_stride = I.boundary_stride; }
+    kern<<<grid, VERIFY_THREADS, 0, I.stream>>>(V, job ? I.enc : EncView{}, I.S, dV);
+    CUDA_TRY(cudaGetLastError());
+  }
+  CUDA_TRY(cudaEventRecord(ev[1], I.stream));
+  if (ybgpu_status s = ReadSmall(&hV, dV, sizeof(JobDev))) return s;
+  float ms = 0;
+  CUDA_TRY(cudaEventElapsedTime(&ms, ev[0], ev[1]));
+  result->gpu_seconds = ms / 1e3;
+  result->entries_parsed = hV.n_counted;
+  if (job) result->bytes_read += I.out_val_bytes + static_cast<uint64_t>(I.n_out) * I.S;
+
+  unsigned long long fail = hV.verify_fail;
+  if (hV.error == DEV_ERR_COMPRESSED) {
+    char buf[160];
+    snprintf(buf, sizeof(buf), "output check: block %u is stored with a compression the engine does not decode", hV.error_where);
+    return Fail(YBGPU_NOT_SUPPORTED, buf);
+  }
+  if (hV.error) fail = std::min(fail, verify_pack(hV.error_where, 0, VERIFY_COMPRESSED));
+  if (fail == ~0ull && job && hV.n_counted != I.n_out) fail = verify_pack(nb, 0, VERIFY_COUNT);
+  if (fail == ~0ull) return YBGPU_OK;
+  result->failure_kind = static_cast<uint32_t>(fail & 15);
+  result->failure_block = static_cast<uint32_t>(fail >> 32);
+  result->failure_entry = static_cast<uint32_t>((fail >> 4) & 0x0fffffffu);
+  char buf[256];
+  snprintf(buf, sizeof(buf), "output check failed: %s at data block %u, entry %u (%llu blocks, %llu entries parsed)", VerifyKindName(result->failure_kind),
+           result->failure_block, result->failure_entry, static_cast<unsigned long long>(nb), static_cast<unsigned long long>(hV.n_counted));
+  return Fail(result->failure_kind == VERIFY_KEY_TOO_LONG ? YBGPU_NOT_SUPPORTED : YBGPU_CORRUPTION, buf);
+}
+
+ybgpu_status Engine::VerifyOutput(ybgpu_output_check* result) {
+  if (!ran_) return Fail(YBGPU_ILLEGAL_STATE, "job has not run");
+  Impl& I = *impl_;
+  CUDA_TRY(cudaSetDevice(opt_.device));
+  ybgpu_status s = VerifyTable(I.out_file, I.out_file_len, I.d_block_off, nullptr, I.n_blocks, opt_.output_key_encoding, true, result);
+  if (s == YBGPU_OK) stats_.path_flags |= YBGPU_PATH_OUTPUT_VERIFIED;
+  return s;
+}
+
+ybgpu_status Engine::VerifySst(const uint8_t* data, uint64_t len, const ybgpu_block_handle* handles, uint64_t nh, int key_encoding,
+                               ybgpu_output_check* result) {
+  Impl& I = *impl_;
+  memset(result, 0, sizeof(*result));
+  if (key_encoding != YBGPU_KEY_ENCODING_SHARED_PREFIX && key_encoding != YBGPU_KEY_ENCODING_THREE_SHARED_PARTS)
+    return Fail(YBGPU_NOT_SUPPORTED, "data block key-value encoding format " + std::to_string(key_encoding) + " is not decoded by the engine");
+  if (nh >= (1ull << 32)) return Fail(YBGPU_NOT_SUPPORTED, "too many data blocks in one file");
+  std::vector<unsigned long long> off(nh); std::vector<uint32_t> sz(nh);
+  for (uint64_t i = 0; i < nh; i++) {
+    if (handles[i].offset > len || handles[i].size > len - handles[i].offset || len - handles[i].offset - handles[i].size < 5)
+      return Fail(YBGPU_CORRUPTION, "block handle outside the data file");
+    if (handles[i].size >= (1ull << 31)) return Fail(YBGPU_NOT_SUPPORTED, "data block too large");
+    off[i] = handles[i].offset; sz[i] = static_cast<uint32_t>(handles[i].size);
+  }
+  if (nh == 0) return YBGPU_OK;
+  CUDA_TRY(cudaSetDevice(opt_.device));
+  VerifyScratch T(I.stream);
+  uint8_t* d = nullptr; unsigned long long* d_off = nullptr; uint32_t* d_sz = nullptr;
+  CUDA_TRY(T.Alloc(&d, len + 64)); CUDA_TRY(T.Alloc(&d_off, nh)); CUDA_TRY(T.Alloc(&d_sz, nh));
+  CUDA_TRY(cudaMemsetAsync(d, 0, 16, I.stream));
+  CUDA_TRY(ChunkedCopyAsync(d + 16, data, len, cudaMemcpyHostToDevice, I.stream));
+  CUDA_TRY(cudaMemsetAsync(d + 16 + len, 0, 48, I.stream));
+  CUDA_TRY(cudaMemcpyAsync(d_off, off.data(), nh * 8, cudaMemcpyHostToDevice, I.stream));
+  CUDA_TRY(cudaMemcpyAsync(d_sz, sz.data(), nh * 4, cudaMemcpyHostToDevice, I.stream));
+  const ybgpu_status s = VerifyTable(d + 16, len, d_off, d_sz, static_cast<uint32_t>(nh), key_encoding, false, result);
+  CUDA_TRY(cudaStreamSynchronize(I.stream));               // the host arrays and the caller's file are free again
+  return s;
 }
 
 }  // namespace ybgpu

@@ -41,6 +41,11 @@ class Engine {
   ybgpu_status FetchFilter(uint8_t* filters, uint8_t* keys, uint32_t* first_entry, uint32_t* block_first);
   // FileMetaData user boundary values (options.compute_user_boundary_values): per range component, min / max value
   ybgpu_status FetchUserValues(ybgpu_user_value* smallest, ybgpu_user_value* largest, uint32_t cap, uint32_t* n);
+  // Output check (verify_kernels.cuh): the finished table of this job, re-read in device memory and compared with the
+  // merge result; and any split SST's data file from host memory (checksums, compressed streams, entries, key order).
+  ybgpu_status VerifyOutput(ybgpu_output_check* result);
+  ybgpu_status VerifySst(const uint8_t* data, uint64_t len, const ybgpu_block_handle* handles, uint64_t nh, int key_encoding,
+                         ybgpu_output_check* result);
   const ybgpu_job_options& options() const { return opt_; }
   ybgpu_job_stats& stats() { return stats_; }
   const std::string& error() const { return error_; }
@@ -55,6 +60,8 @@ class Engine {
   ybgpu_status UploadSmall(void* dev_dst, const void* host_src, size_t n);
   ybgpu_status ReadViaMapped(void* host_dst, const void* dev_src, size_t row_bytes, size_t src_pitch, size_t rows);
   ybgpu_status EnsureKvStream();
+  ybgpu_status VerifyTable(const uint8_t* file, uint64_t file_len, const unsigned long long* d_off, const uint32_t* d_size,
+                           uint32_t nb, int key_encoding, bool job, ybgpu_output_check* result);
   struct Impl;
   ybgpu_job_options opt_;
   Impl* impl_;

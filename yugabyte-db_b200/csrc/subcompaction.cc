@@ -314,7 +314,7 @@ ybgpu_status CompactFilesCore(const ybgpu_job_options* options, const ybgpu_inpu
                               uint32_t max_subcompactions, uint32_t max_in_flight,
                               uint8_t* data_arena, uint64_t data_arena_cap, uint8_t* meta_arena, uint64_t meta_arena_cap,
                               const volatile int32_t* shutting_down, ybgpu_sub_output* outputs, uint32_t* num_outputs,
-                              ybgpu_job_stats* total, char* err, uint64_t err_cap, OneTable* one) {
+                              ybgpu_job_stats* total, char* err, uint64_t err_cap, OneTable* one, bool verify_outputs) {
   auto fail = [&](ybgpu_status s, const std::string& msg) {
     if (err && err_cap) snprintf(err, err_cap, "%s", msg.c_str());
     return s;
@@ -525,6 +525,13 @@ ybgpu_status CompactFilesCore(const ybgpu_job_options* options, const ybgpu_inpu
     if (added) {
       s = ybgpu_job_run(job, shutting_down);
       if (s != YBGPU_OK) { job_fail(s, "run"); return; }
+      if (verify_outputs) {
+        // paranoid_file_checks: the range's table is re-read on its own stream while it is still in device memory; a bad
+        // range fails the compaction before a byte of it reaches the caller's arena
+        ybgpu_output_check chk;
+        s = ybgpu_job_verify_output(job, &chk);
+        if (s != YBGPU_OK) { job_fail(s, "verify_output"); return; }
+      }
       t_ran = ms_now();
       uint64_t dl = 0, ml = 0;
       s = ybgpu_job_output_sizes(job, &dl, &ml);
@@ -639,14 +646,14 @@ ybgpu_status ybgpu_compact_files(const ybgpu_job_options* options, const ybgpu_i
                                  const volatile int32_t* shutting_down, ybgpu_sub_output* outputs, uint32_t* num_outputs,
                                  ybgpu_job_stats* total, char* err, uint64_t err_cap) {
   return CompactFilesCore(options, files, num_files, max_subcompactions, max_in_flight, data_arena, data_arena_cap, meta_arena,
-                          meta_arena_cap, shutting_down, outputs, num_outputs, total, err, err_cap, nullptr);
+                          meta_arena_cap, shutting_down, outputs, num_outputs, total, err, err_cap, nullptr, false);
 }
 
-ybgpu_status ybgpu_compact_files_one_table(const ybgpu_job_options* options, const ybgpu_input_file* files, uint32_t num_files,
+static ybgpu_status CompactFilesOneTable(const ybgpu_job_options* options, const ybgpu_input_file* files, uint32_t num_files,
                                            uint32_t max_subcompactions, uint32_t max_in_flight,
                                            uint8_t* data_out, uint64_t data_cap, uint8_t* meta_out, uint64_t meta_cap,
                                            const volatile int32_t* shutting_down, ybgpu_one_table_result* result,
-                                           ybgpu_job_stats* total, char* err, uint64_t err_cap) {
+                                           ybgpu_job_stats* total, char* err, uint64_t err_cap, bool verify_outputs) {
   if (!result || !data_out || !meta_out) { if (err && err_cap) snprintf(err, err_cap, "null argument"); return YBGPU_INVALID_ARGUMENT; }
   memset(result, 0, sizeof(*result));
   if (max_subcompactions == 0) max_subcompactions = 1;
@@ -655,7 +662,7 @@ ybgpu_status ybgpu_compact_files_one_table(const ybgpu_job_options* options, con
   OneTable one;
   ybgpu_job_stats tot;
   ybgpu_status s = CompactFilesCore(options, files, num_files, max_subcompactions, max_in_flight, data_out, data_cap, nullptr, 0,
-                                    shutting_down, outs.data(), &n, &tot, err, err_cap, &one);
+                                    shutting_down, outs.data(), &n, &tot, err, err_cap, &one, verify_outputs);
   if (s != YBGPU_OK) return s;
   if (one.meta.size() > meta_cap) { if (err && err_cap) snprintf(err, err_cap, "metadata buffer too small"); return YBGPU_INVALID_ARGUMENT; }
   memcpy(meta_out, one.meta.data(), one.meta.size());
@@ -668,6 +675,33 @@ ybgpu_status ybgpu_compact_files_one_table(const ybgpu_job_options* options, con
   tot.output_data_file_size = one.data_len; tot.output_meta_file_size = one.meta.size();
   if (total) *total = tot;
   return YBGPU_OK;
+}
+
+ybgpu_status ybgpu_compact_files_one_table(const ybgpu_job_options* options, const ybgpu_input_file* files, uint32_t num_files,
+                                           uint32_t max_subcompactions, uint32_t max_in_flight,
+                                           uint8_t* data_out, uint64_t data_cap, uint8_t* meta_out, uint64_t meta_cap,
+                                           const volatile int32_t* shutting_down, ybgpu_one_table_result* result,
+                                           ybgpu_job_stats* total, char* err, uint64_t err_cap) {
+  return CompactFilesOneTable(options, files, num_files, max_subcompactions, max_in_flight, data_out, data_cap, meta_out, meta_cap, shutting_down,
+                              result, total, err, err_cap, false);
+}
+
+ybgpu_status ybgpu_compact_files_checked(const ybgpu_job_options* options, const ybgpu_input_file* files, uint32_t num_files,
+                                         uint32_t max_subcompactions, uint32_t max_in_flight,
+                                         uint8_t* data_arena, uint64_t data_arena_cap, uint8_t* meta_arena, uint64_t meta_arena_cap,
+                                         const volatile int32_t* shutting_down, ybgpu_sub_output* outputs, uint32_t* num_outputs,
+                                         ybgpu_job_stats* total, char* err, uint64_t err_cap, int32_t verify_outputs) {
+  return CompactFilesCore(options, files, num_files, max_subcompactions, max_in_flight, data_arena, data_arena_cap, meta_arena,
+                          meta_arena_cap, shutting_down, outputs, num_outputs, total, err, err_cap, nullptr, verify_outputs != 0);
+}
+
+ybgpu_status ybgpu_compact_files_one_table_checked(const ybgpu_job_options* options, const ybgpu_input_file* files, uint32_t num_files,
+                                                   uint32_t max_subcompactions, uint32_t max_in_flight,
+                                                   uint8_t* data_out, uint64_t data_cap, uint8_t* meta_out, uint64_t meta_cap,
+                                                   const volatile int32_t* shutting_down, ybgpu_one_table_result* result,
+                                                   ybgpu_job_stats* total, char* err, uint64_t err_cap, int32_t verify_outputs) {
+  return CompactFilesOneTable(options, files, num_files, max_subcompactions, max_in_flight, data_out, data_cap, meta_out, meta_cap, shutting_down,
+                              result, total, err, err_cap, verify_outputs != 0);
 }
 
 }  // extern "C"
