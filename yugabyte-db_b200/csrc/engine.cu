@@ -1501,6 +1501,7 @@ struct Engine::Impl {
   JobDev hJ{};
   // K4/K5 state kept for lazy result fetches
   Desc* d_desc = nullptr; Sums3* d_partial = nullptr; ValueRewrite* d_rw = nullptr;
+  bool partial_ready = false;   // d_partial holds the scanned chunk sums (computed when survivors are compacted or the KV stream is fetched)
   uint64_t N = 0; int S = 0; uint32_t n_chunks = 0;
   bool kv_emitted = false;
   Desc* d_kept = nullptr;
@@ -2387,10 +2388,10 @@ ybgpu_status Engine::Run(const volatile int32_t* shutting_down) {
   const uint32_t n_chunks = static_cast<uint32_t>((N + EMIT_CHUNK - 1) / EMIT_CHUNK);
   Sums3* d_partial = nullptr;
   CUDA_TRY(DevAlloc(&I.allocs, &d_partial, n_chunks + 1));
-  k_emit_sums<<<n_chunks, EMIT_THREADS, 0, I.stream>>>(d_desc, N, d_partial);
-  k_scan_sums<<<1, 1024, 0, I.stream>>>(d_partial, n_chunks);
-  launches += 2;
   I.d_desc = d_desc; I.d_partial = d_partial; I.d_rw = d_rw; I.N = N; I.S = Sfinal; I.n_chunks = n_chunks;
+  // the chunk sums place survivors among dropped entries: k_compact_desc needs them now, k_emit when the KV stream is asked for
+  I.partial_ready = false;
+  if (I.n_out != N) { if (ybgpu_status s = EnsureChunkSums()) return s; launches += 2; }
   if (I.n_out >= (1ull << 32)) return Fail(YBGPU_NOT_SUPPORTED, "too many output entries");
   const uint32_t n = static_cast<uint32_t>(I.n_out);
   if (n) {
@@ -2426,52 +2427,55 @@ ybgpu_status Engine::Run(const volatile int32_t* shutting_down) {
     }
     CUDA_TRY(DevAlloc(&I.allocs, &E.max_add, 1));
     CUDA_TRY(cudaMemsetAsync(E.max_add, 0, 4, I.stream));
-    k_entry_sizes<<<GridFor(n, 256, sms), 256, 0, I.stream>>>(E, Sfinal);
-    // P
+    // ---- block planning: per-entry sizes with the chunk partials of P, QQ and the filter-key ordinals in one pass, one scan
+    // launch over all partial arrays, one launch that applies them (encode_kernels.cuh)
     const uint32_t pc = (n + SCAN_CHUNK - 1) / SCAN_CHUNK;
-    unsigned long long* d_pp = nullptr;
-    CUDA_TRY(DevAlloc(&I.allocs, &d_pp, pc + 1));
-    k_p_sums<<<pc, 256, 0, I.stream>>>(E.nr, n, d_pp);
-    k_scan_u64_single<<<1, 1024, 0, I.stream>>>(d_pp, pc, nullptr);
-    k_p_final<<<pc, 256, 0, I.stream>>>(E.nr, n, d_pp, E.P);
-    // QQ
     const uint32_t rows = (n + ri - 1) / ri;
     const uint32_t qchunks = (rows + QROWS - 1) / QROWS;
-    unsigned long long* d_qp = nullptr;
+    unsigned long long *d_pp = nullptr, *d_qp = nullptr;
+    uint32_t* d_counts = nullptr;                         // [0] data blocks, [1] distinct filter keys
+    uint8_t* d_is_new = nullptr; uint32_t* d_npart = nullptr; uint32_t* d_new_entry = nullptr; uint32_t* d_hash = nullptr;
+    CUDA_TRY(DevAlloc(&I.allocs, &d_pp, pc + 1));
     CUDA_TRY(DevAlloc(&I.allocs, &d_qp, static_cast<size_t>(qchunks) * ri + 1));
-    const uint32_t qthreads = qchunks * ri;
-    k_qq_sums<<<(qthreads + 255) / 256, 256, 0, I.stream>>>(E.D, n, ri, d_qp, qchunks);
-    k_scan_u64_single<<<ri, 1024, 0, I.stream>>>(d_qp, qchunks, nullptr, qchunks);   // one residue class per CTA
-    k_qq_final<<<(qthreads + 255) / 256, 256, 0, I.stream>>>(E.D, n, ri, d_qp, qchunks, E.QQ);
-    launches += 8;
+    CUDA_TRY(DevAlloc(&I.allocs, &d_counts, 2));
+    CUDA_TRY(cudaMemsetAsync(d_counts, 0, 8, I.stream));
+    host::FilterGeometry hg{};
+    if (E.fk_len) {
+      hg = host::ComputeFilterGeometry(opt_.filter_block_size ? opt_.filter_block_size : 65536u);
+      if (hg.max_keys == 0) return Fail(YBGPU_INVALID_ARGUMENT, "filter_block_size too small");
+      CUDA_TRY(DevAlloc(&I.allocs, &d_is_new, n)); CUDA_TRY(DevAlloc(&I.allocs, &d_npart, pc + 1));
+      // no more distinct filter keys than entries: sized before the count is known, so that one pass can fill both
+      CUDA_TRY(DevAlloc(&I.allocs, &d_new_entry, static_cast<size_t>(n) + 1));
+      if (((hg.filter_bytes + 7u) & ~7u) <= FILTER_SMEM_MAX) CUDA_TRY(DevAlloc(&I.allocs, &d_hash, n));
+    }
+    k_plan_entries<<<(n + PLAN_CHUNK - 1) / PLAN_CHUNK, 256, 0, I.stream>>>(E, Sfinal, d_is_new, d_pp, pc, d_qp, qchunks, d_npart);
+    k_plan_scan<<<ri + 2, 1024, 0, I.stream>>>(d_pp, pc, d_qp, qchunks, d_npart, d_counts + 1);
+    k_plan_final<<<pc + (qchunks * ri + 255) / 256, 256, 0, I.stream>>>(E, Sfinal, d_is_new, d_pp, pc, d_qp, qchunks, d_npart, d_new_entry, d_hash);
+    launches += 3;
     // block cuts
-    k_next<<<GridFor(n, 256, sms), 256, 0, I.stream>>>(E);
     const uint32_t nsegs = (n + SEG - 1) / SEG;
     const uint32_t ngroups = (nsegs + GROUP_SEGS - 1) / GROUP_SEGS;
-    uint32_t *d_gexit = nullptr, *d_group_first = nullptr, *d_seg_first = nullptr, *d_spart = nullptr, *d_nblocks = nullptr;
-    uint8_t* d_is_start = nullptr;
+    uint32_t *d_gexit = nullptr, *d_group_first = nullptr, *d_seg_first = nullptr, *d_seg_blocks = nullptr;
     CUDA_TRY(DevAlloc(&I.allocs, &d_gexit, static_cast<size_t>(ngroups) * SEG));
     CUDA_TRY(DevAlloc(&I.allocs, &d_group_first, ngroups)); CUDA_TRY(DevAlloc(&I.allocs, &d_seg_first, nsegs));
-    CUDA_TRY(DevAlloc(&I.allocs, &d_is_start, n)); CUDA_TRY(DevAlloc(&I.allocs, &d_spart, pc + 1)); CUDA_TRY(DevAlloc(&I.allocs, &d_nblocks, 1));
-    CUDA_TRY(cudaMemsetAsync(d_is_start, 0, n, I.stream));
+    CUDA_TRY(DevAlloc(&I.allocs, &d_seg_blocks, nsegs));
     k_seg_exit<<<nsegs, 256, 0, I.stream>>>(E);
     k_group_exit<<<static_cast<uint32_t>((static_cast<uint64_t>(ngroups) * SEG + 255) / 256), 256, 0, I.stream>>>(E, d_gexit, ngroups);
     k_chain_groups<<<1, 32, 0, I.stream>>>(E, d_gexit, ngroups, d_group_first);
     k_group_fill<<<(ngroups + 127) / 128, 128, 0, I.stream>>>(E, d_group_first, ngroups, d_seg_first, nsegs);
-    k_mark_starts<<<(nsegs + 127) / 128, 128, 0, I.stream>>>(E, d_seg_first, nsegs, d_is_start);
-    k_start_sums<<<pc, 256, 0, I.stream>>>(d_is_start, n, d_spart);
-    k_scan_u32_single<<<1, 1024, 0, I.stream>>>(d_spart, pc, d_nblocks);
-    launches += 8;
-    uint32_t nblocks = 0;
-    if (ybgpu_status s = ReadSmall(&nblocks, d_nblocks, 4)) return s;
+    k_count_starts<<<(nsegs + 127) / 128, 128, 0, I.stream>>>(E, d_seg_first, nsegs, d_seg_blocks);
+    k_scan_u32_single<<<1, 1024, 0, I.stream>>>(d_seg_blocks, nsegs, d_counts);
+    launches += 6;
+    uint32_t counts[2] = {0, 0};
+    if (ybgpu_status s = ReadSmall(counts, d_counts, 8)) return s;
+    const uint32_t nblocks = counts[0], n_keys = counts[1];
     I.n_blocks = nblocks;
     CUDA_TRY(DevAlloc(&I.allocs, &I.d_block_first, static_cast<size_t>(nblocks) + 1));
     CUDA_TRY(DevAlloc(&I.allocs, &I.d_block_off, static_cast<size_t>(nblocks) + 1));
     unsigned long long* d_total = nullptr;                // [0] file length, [1] largest block (contents + trailer)
     CUDA_TRY(DevAlloc(&I.allocs, &d_total, 2));
     CUDA_TRY(cudaMemsetAsync(d_total, 0, 16, I.stream));
-    k_block_first<<<pc, 256, 0, I.stream>>>(d_is_start, n, d_spart, I.d_block_first);
-    k_block_sizes<<<GridFor(nblocks, 256, sms), 256, 0, I.stream>>>(E, I.d_block_first, nblocks, I.d_block_off, d_total + 1);
+    k_block_fill<<<(nsegs + 127) / 128, 128, 0, I.stream>>>(E, d_seg_first, nsegs, d_seg_blocks, I.d_block_first, I.d_block_off, d_total + 1);
     {
       const uint32_t bc = (nblocks + SCAN_CHUNK - 1) / SCAN_CHUNK;
       unsigned long long* d_bpart = nullptr;
@@ -2479,7 +2483,7 @@ ybgpu_status Engine::Run(const volatile int32_t* shutting_down) {
       k_u64_chunk_sums<<<bc, 256, 0, I.stream>>>(I.d_block_off, nblocks, d_bpart);
       k_scan_u64_single<<<1, 1024, 0, I.stream>>>(d_bpart, bc, d_total);
       k_u64_chunk_final<<<bc, 256, 0, I.stream>>>(I.d_block_off, nblocks, d_bpart);
-      launches += 2;
+      launches += 4;
     }
     unsigned long long total_and_max[2] = {0, 0};
     if (ybgpu_status s = ReadSmall(total_and_max, d_total, 16)) return s;
@@ -2593,41 +2597,26 @@ ybgpu_status Engine::Run(const volatile int32_t* shutting_down) {
     }
     if (E.fk_len) {
       // ---- bloom filter blocks: distinct filter keys -> ordinals -> 64 KB blocks of max_keys keys each
-      const host::FilterGeometry hg = host::ComputeFilterGeometry(opt_.filter_block_size ? opt_.filter_block_size : 65536u);
       BloomGeometry g{hg.num_lines, hg.num_probes, hg.max_keys, hg.filter_bytes, (hg.filter_bytes + 7u) & ~7u};
-      if (g.max_keys == 0) return Fail(YBGPU_INVALID_ARGUMENT, "filter_block_size too small");
-      uint8_t* d_is_new = nullptr; uint32_t* d_npart = nullptr; uint32_t* d_nkeys = nullptr; uint32_t* d_new_entry = nullptr;
-      CUDA_TRY(DevAlloc(&I.allocs, &d_is_new, n)); CUDA_TRY(DevAlloc(&I.allocs, &d_npart, pc + 1)); CUDA_TRY(DevAlloc(&I.allocs, &d_nkeys, 1));
-      k_filter_new<<<GridFor(n, 256, sms), 256, 0, I.stream>>>(E, Sfinal, d_is_new);
-      k_start_sums<<<pc, 256, 0, I.stream>>>(d_is_new, n, d_npart);
-      k_scan_u32_single<<<1, 1024, 0, I.stream>>>(d_npart, pc, d_nkeys);
-      uint32_t n_keys = 0;
-      if (ybgpu_status s = ReadSmall(&n_keys, d_nkeys, 4)) return s;
       // a (possibly empty) block is always flushed at Finish (block_based_table_builder.cc:768-770)
       const uint32_t nfb = std::max<uint32_t>(1, (n_keys + g.max_keys - 1) / g.max_keys);
       I.n_filter_blocks = nfb; I.filter_block_bytes = g.block_bytes;
       I.filter_key_stride = static_cast<uint32_t>((max_ikey + 2 + 7) & ~7u);
-      CUDA_TRY(DevAlloc(&I.allocs, &d_new_entry, static_cast<size_t>(n_keys) + 1));
       CUDA_TRY(DevAlloc(&I.allocs, &I.d_filters, static_cast<size_t>(nfb) * g.dev_stride + 16));
       CUDA_TRY(DevAlloc(&I.allocs, &I.d_filter_keys, static_cast<size_t>(nfb) * 2 * I.filter_key_stride));
       CUDA_TRY(DevAlloc(&I.allocs, &I.d_filter_first, nfb));
       CUDA_TRY(cudaMemsetAsync(I.d_filters, 0, static_cast<size_t>(nfb) * g.dev_stride, I.stream));
-      k_block_first<<<pc, 256, 0, I.stream>>>(d_is_new, n, d_npart, d_new_entry);
-      if (n_keys && g.dev_stride <= FILTER_SMEM_MAX) {
+      if (n_keys && d_hash) {
         CUDA_TRY(cudaFuncSetAttribute(k_filter_build_smem, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(g.dev_stride)));
         const uint32_t resident = std::max<uint32_t>(1, std::min<uint32_t>(2, (200u * 1024u) / (g.dev_stride + 1024u))) * sms;   // CTAs that fit at once
         const uint32_t parts = std::max<uint32_t>(1, std::min<uint32_t>(8, resident / nfb));
-        uint32_t* d_hash = nullptr;
-        CUDA_TRY(DevAlloc(&I.allocs, &d_hash, n_keys));
-        k_filter_hash<<<GridFor(n_keys, 256, sms), 256, 0, I.stream>>>(E, Sfinal, d_new_entry, n_keys, d_hash);
         k_filter_build_smem<<<std::min<uint32_t>(nfb * parts, resident * 4), 1024, g.dev_stride, I.stream>>>(d_hash, n_keys, g, nfb, parts, I.d_filters);
-        launches++;
       } else if (n_keys) {
         k_filter_build<<<GridFor(n_keys, 256, sms), 256, 0, I.stream>>>(E, Sfinal, d_new_entry, n_keys, g, I.d_filters);
       }
       k_filter_finish<<<GridFor(static_cast<uint64_t>(nfb) * 2, 256, sms), 256, 0, I.stream>>>(E, Sfinal, d_new_entry, n_keys, g, nfb, I.d_filters,
                                                                                               I.d_filter_keys, I.filter_key_stride, I.d_filter_first);
-      launches += 5 + (n_keys ? 1 : 0);
+      launches += 1 + (n_keys ? 1 : 0);
     }
     if (opt_.compute_user_boundary_values && opt_.retention_enabled) {
       const int bgrid = static_cast<int>(std::max<uint64_t>(1, std::min<uint64_t>((n + 255) / 256, static_cast<uint64_t>(sms) * 2)));
@@ -2644,7 +2633,7 @@ ybgpu_status Engine::Run(const volatile int32_t* shutting_down) {
     // slot 2*nblocks (one past the per-block pairs): the first key of the file (FileMetaData::smallest)
     CUDA_TRY(DevAlloc(&I.allocs, &I.d_boundary, (static_cast<size_t>(nblocks) * 2 + 1) * I.boundary_stride));
     k_boundary_keys<<<GridFor(static_cast<uint64_t>(nblocks) * 2 + 1, 256, sms), 256, 0, I.stream>>>(E, Sfinal, I.d_block_first, nblocks, I.d_boundary, I.boundary_stride);
-    launches += 4;
+    launches++;
   }
   CUDA_TRY(end_phase());
   CUDA_TRY(cudaEventRecord(I.ev1, I.stream));
@@ -2699,6 +2688,16 @@ ybgpu_status Engine::KvStreamSizes(uint64_t* n, uint64_t* kb, uint64_t* vb) cons
   return YBGPU_OK;
 }
 
+// Exclusive chunk sums (survivors, key bytes, value bytes) of the merged-order descriptors: two launches on the job's stream.
+ybgpu_status Engine::EnsureChunkSums() {
+  Impl& I = *impl_;
+  k_emit_sums<<<I.n_chunks, EMIT_THREADS, 0, I.stream>>>(I.d_desc, I.N, I.d_partial);
+  k_scan_sums<<<1, 1024, 0, I.stream>>>(I.d_partial, I.n_chunks);
+  I.partial_ready = true;
+  CUDA_TRY(cudaGetLastError());
+  return YBGPU_OK;
+}
+
 // The flat KV stream (what CompactionFeed::Feed consumers want) is materialised on demand.
 ybgpu_status Engine::EnsureKvStream() {
   Impl& I = *impl_;
@@ -2710,6 +2709,7 @@ ybgpu_status Engine::EnsureKvStream() {
   CUDA_TRY(DevAlloc(&I.allocs, &I.out_koff, I.n_out + 1));
   CUDA_TRY(DevAlloc(&I.allocs, &I.out_voff, I.n_out + 1));
   if (I.N) {
+    if (!I.partial_ready) { if (ybgpu_status s = EnsureChunkSums()) return s; stats_.gpu_kernel_launches += 2; }
     EmitView ev{};
     ev.runs = I.dRuns; ev.desc = I.d_desc; ev.partial = I.d_partial; ev.rewrites = I.d_rw;
     ev.out_keys = I.out_keys; ev.out_koff = I.out_koff; ev.out_vals = I.out_vals; ev.out_voff = I.out_voff; ev.N = I.N;

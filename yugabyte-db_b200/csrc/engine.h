@@ -60,6 +60,7 @@ class Engine {
   ybgpu_status UploadSmall(void* dev_dst, const void* host_src, size_t n);
   ybgpu_status ReadViaMapped(void* host_dst, const void* dev_src, size_t row_bytes, size_t src_pitch, size_t rows);
   ybgpu_status EnsureKvStream();
+  ybgpu_status EnsureChunkSums();
   ybgpu_status VerifyTable(const uint8_t* file, uint64_t file_len, const unsigned long long* d_off, const uint32_t* d_size,
                            uint32_t nb, int key_encoding, bool job, ybgpu_output_check* result);
   struct Impl;
