@@ -1568,6 +1568,7 @@ __global__ void __launch_bounds__(ENC_THREADS, 4) k_encode_v4(EncView E, int S, 
 //   * the warp then walks the round's entries two at a time, one per half-warp: the gap goes scratch -> HBM, the value
 //     HBM -> registers -> HBM as destination-aligned 16-byte chunks (one per lane, two aligned source vectors funnel-
 //     shifted into place), the <= 15 bytes in front of the first / behind the last full chunk as one byte per lane;
+//     each step's value loads are issued one step ahead of its stores;
 //   * the block checksum is the same GF(2)-linear combination as in v4 — every gap, value and restart-array word
 //     enters as (raw CRC) * x^(8 * bytes behind it), XOR-accumulated unreduced per lane — so no byte of the block is
 //     read back.
@@ -1584,6 +1585,57 @@ __device__ __forceinline__ uint32_t enc5_xpow(unsigned long long nbytes) {
 __device__ __forceinline__ void enc5_prefetch_l2(const void* p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
 __device__ __forceinline__ void enc5_store_u32(uint8_t* p, uint32_t v) {
   p[0] = static_cast<uint8_t>(v); p[1] = static_cast<uint8_t>(v >> 8); p[2] = static_cast<uint8_t>(v >> 16); p[3] = static_cast<uint8_t>(v >> 24);
+}
+
+// One walk step of a half-warp: lane hl's share of a copied value (vd = its destination, len bytes from src). Loads:
+// the first destination-aligned 16-byte chunk of the lane (two aligned source vectors, funnel-shifted at the store),
+// one byte in front of the first / behind the last full chunk (a value without a full chunk: bytes hl and hl + 16).
+// enc5_put stores them, and the further chunks of a value longer than 16 chunks.
+struct Enc5Pre { uint4 a, b; uint32_t x; };          // x = source shift | head byte << 8 | tail byte << 16
+__device__ __forceinline__ Enc5Pre enc5_fetch(const uint8_t* vd, const uint8_t* src, uint32_t len, uint32_t hl) {
+  Enc5Pre t;
+  t.a = make_uint4(0, 0, 0, 0); t.b = t.a;
+  uint32_t sh = 0, hb = 0, tb = 0;
+  if (len) {
+    const uintptr_t d0 = reinterpret_cast<uintptr_t>(vd), d1 = d0 + len;
+    const uintptr_t fa = (d0 + 15) & ~static_cast<uintptr_t>(15), fb = d1 & ~static_cast<uintptr_t>(15);
+    if (fb > fa) {
+      if (d0 + hl < fa) hb = __ldg(src + hl);
+      if (fb + hl < d1) tb = __ldg(src + (fb - d0) + hl);
+      const uintptr_t A = fa + 16u * hl;
+      if (A < fb) {
+        const uint8_t* s = src + (A - d0);
+        sh = static_cast<uint32_t>(reinterpret_cast<uintptr_t>(s) & 15);
+        const uint4* v = reinterpret_cast<const uint4*>(s - sh);
+        t.a = __ldg(v);
+        if (sh) t.b = __ldg(v + 1);
+      }
+    } else {
+      if (hl < len) hb = __ldg(src + hl);
+      if (hl + 16 < len) tb = __ldg(src + hl + 16);
+    }
+  }
+  t.x = sh | (hb << 8) | (tb << 16);
+  return t;
+}
+__device__ __forceinline__ void enc5_put(const Enc5Pre& t, uint8_t* vd, const uint8_t* src, uint32_t len, uint32_t hl) {
+  if (!len) return;
+  const uint8_t hb = static_cast<uint8_t>(t.x >> 8), tb = static_cast<uint8_t>(t.x >> 16);
+  const uintptr_t d0 = reinterpret_cast<uintptr_t>(vd), d1 = d0 + len;
+  const uintptr_t fa = (d0 + 15) & ~static_cast<uintptr_t>(15), fb = d1 & ~static_cast<uintptr_t>(15);
+  if (fb > fa) {
+    if (d0 + hl < fa) vd[hl] = hb;
+    if (fb + hl < d1) *reinterpret_cast<uint8_t*>(fb + hl) = tb;
+    uintptr_t A = fa + 16u * hl;
+    if (A < fb) {
+      const uint32_t sh = t.x & 15;
+      *reinterpret_cast<uint4*>(A) = sh ? shift16(t.a, t.b, sh) : t.a;
+      for (A += 256; A < fb; A += 256) copy_chunk16(reinterpret_cast<uint8_t*>(A), src + (A - d0));
+    }
+  } else {
+    if (hl < len) vd[hl] = hb;
+    if (hl + 16 < len) vd[hl + 16] = tb;
+  }
 }
 
 template <int ENC>
@@ -1668,35 +1720,37 @@ __global__ void __launch_bounds__(ENC5_THREADS, ENC == 1 ? 4 : 2) k_encode_v5(En
         const RunView& rn = E.runs[d_next.run];
         enc5_prefetch_l2(rn.rec + static_cast<size_t>(d_next.gid - rn.gid_base) * S);
       }
+      // The warp walks the round's entries two at a time, one per half-warp, software-pipelined: the value loads of the
+      // next step are issued before this step's stores, so that a step's stores wait on no load of their own (a 64-
+      // register budget holds one step ahead; two ahead spill and were slower).
       const uint32_t nact = min(32u, e - r0);
-#pragma unroll 2
-      for (uint32_t q0 = 0; q0 < nact; q0 += 2) {
-        const uint32_t q = q0 + half;
+      const uint32_t nsteps = (nact + 1) >> 1;
+      auto step_args = [&](uint32_t st, uint8_t*& gdst, const uint8_t*& src, uint32_t& gap, uint32_t& len) {
+        const uint32_t q = 2 * st + half;
         const unsigned long long eoff_q = __shfl_sync(0xffffffffu, eoff, q & 31);
-        const unsigned long long src_q = __shfl_sync(0xffffffffu, srcp, q & 31);
-        const uint32_t gap_q = __shfl_sync(0xffffffffu, gap_len, q & 31);
-        const uint32_t len_q = __shfl_sync(0xffffffffu, copy_len, q & 31);
-        if (q >= nact) continue;
-        uint8_t* gdst = blk + eoff_q;
-        {
-          const uint8_t* scq = wsc + q * G + ((4u - (gap_q & 3u)) & 3u);
-          if (hl < gap_q) gdst[hl] = scq[hl];
-          if (hl + 16 < gap_q) gdst[hl + 16] = scq[hl + 16];
-          for (uint32_t i = hl + 32; i < gap_q; i += 16) gdst[i] = scq[i];
-        }
-        if (len_q) {
-          const uint8_t* src = reinterpret_cast<const uint8_t*>(src_q);
-          uint8_t* vd = gdst + gap_q;
-          const uintptr_t d0 = reinterpret_cast<uintptr_t>(vd), d1 = d0 + len_q;
-          const uintptr_t fa = (d0 + 15) & ~static_cast<uintptr_t>(15), fb = d1 & ~static_cast<uintptr_t>(15);
-          if (fb > fa) {
-            if (d0 + hl < fa) vd[hl] = __ldg(src + hl);
-            if (fb + hl < d1) *reinterpret_cast<uint8_t*>(fb + hl) = __ldg(src + (fb - d0) + hl);
-            for (uintptr_t A = fa + 16u * hl; A < fb; A += 256) copy_chunk16(reinterpret_cast<uint8_t*>(A), src + (A - d0));
-          } else {
-            for (uint32_t i = hl; i < len_q; i += 16) vd[i] = __ldg(src + i);
-          }
-        }
+        src = reinterpret_cast<const uint8_t*>(__shfl_sync(0xffffffffu, srcp, q & 31));
+        gap = __shfl_sync(0xffffffffu, gap_len, q & 31);
+        len = __shfl_sync(0xffffffffu, copy_len, q & 31);
+        gdst = blk + eoff_q;
+        if (q >= nact) { gap = 0; len = 0; }
+      };
+      Enc5Pre pre;
+      {
+        uint8_t* gdst; const uint8_t* src; uint32_t gap, len;
+        step_args(0, gdst, src, gap, len);
+        pre = enc5_fetch(gdst + gap, src, len, hl);
+      }
+      for (uint32_t st = 0; st < nsteps; st++) {
+        uint8_t* gdst; const uint8_t* src; uint32_t gap, len;
+        step_args(st + 1, gdst, src, gap, len);
+        const Enc5Pre nx = enc5_fetch(gdst + gap, src, st + 1 < nsteps ? len : 0u, hl);
+        step_args(st, gdst, src, gap, len);
+        const uint8_t* scq = wsc + (2 * st + half) * G + ((4u - (gap & 3u)) & 3u);
+        if (hl < gap) gdst[hl] = scq[hl];
+        if (hl + 16 < gap) gdst[hl + 16] = scq[hl + 16];
+        for (uint32_t i = hl + 32; i < gap; i += 16) gdst[i] = scq[i];
+        enc5_put(pre, gdst + gap, src, len, hl);
+        pre = nx;
       }
       d_cur = d_next;
       __syncwarp();                                // the scratch rows are rewritten by the next round
