@@ -136,6 +136,18 @@ typedef struct ybgpu_job_options {
    * (tests: liblz4, pyarrow's lz4_raw). Any other value is NotSupported at job creation (ybgpu_job_create,
    * ybgpu_compact_files*, ybgpu_compact_range_sharded, ybgpu_table_builder_create) before the device is touched. */
   int32_t output_compression;        /* YBGPU_COMPRESSION_* ; default none */
+
+  /* --- device memory (INTEGRATION.md section 3 "Device memory") --- bytes of HBM the job may hold at once; 0 = unlimited
+   * (the default). Every device allocation of a job (inputs, decode and merge arrays, the output table, the output check's
+   * temporaries) is counted at its requested size, the engine's 32-byte pads included; the stream-ordered pool's own
+   * rounding is not. add_input* and run first check on the host what is already known — the inputs' device copies plus,
+   * when any input block is stored compressed, the uncompressed image (sum of the blocks' varint32 preambles) — and
+   * refuse with YBGPU_NOT_SUPPORTED ("device memory budget exceeded ...", need and budget) before anything is uploaded.
+   * An allocation during run that would pass the budget fails the job with YBGPU_RUNTIME_ERROR and the message
+   * "device memory budget exceeded: need N, in use U, budget B"; the job's stream is drained first, so no kernel of it
+   * is left running, and destroy returns every byte to the pool. Pipelined calls (ybgpu_compact_files*) take it as the
+   * budget of the whole compaction. ybgpu_job_stats::device_bytes_peak reports the high-water mark either way. */
+  uint64_t device_memory_budget;
 } ybgpu_job_options;
 
 void ybgpu_job_options_init(ybgpu_job_options* o);   /* reference defaults */
@@ -177,6 +189,11 @@ typedef struct ybgpu_job_stats {
   /* which kernels ran (diagnostics, tests): YBGPU_PATH_* bits; summed over the ranges of a pipelined compaction */
   uint32_t path_flags;
   uint32_t tiles_inside_rows;          /* merge tiles that started inside a row group larger than a tile */
+  /* high-water mark of the job's device bytes in use (requested sizes, 32-byte pads included, the pool's rounding not:
+   * cudaMemPoolAttrUsedMemHigh of a job alone on its device is at least this, larger by the pool's granularity); for a
+   * pipelined compaction, the high-water mark of the bytes all its ranges hold at once (every allocation and free of
+   * every range updates one shared count), not the sum of the ranges' own peaks */
+  uint64_t device_bytes_peak;
 } ybgpu_job_stats;
 enum {
   YBGPU_PATH_FUSED_INGEST = 1,         /* k_ingest: TMA-staged verify + value CRCs + decode in one pass */
@@ -335,18 +352,39 @@ ybgpu_status ybgpu_plan_subcompactions(const ybgpu_input_file* files, uint32_t n
                                        int32_t docdb_keys, uint8_t* splitters, uint32_t* splitter_lens,
                                        uint32_t* num_splitters);
 
+/* The row-aligned splitter that cuts the key range [lower, upper) (len 0 = unbounded) of the inputs in two halves of about
+ * equal block bytes: the planner of ybgpu_plan_subcompactions on the range's slice. It lies strictly inside the range.
+ * YBGPU_NOT_FOUND: no row boundary lies inside (the range holds one row, or no index separator falls inside it).
+ * splitter: 256 bytes. */
+ybgpu_status ybgpu_split_range(const ybgpu_input_file* files, uint32_t num_files, int32_t docdb_keys, const uint8_t* lower,
+                               uint32_t lower_len, const uint8_t* upper, uint32_t upper_len, uint8_t* splitter, uint32_t* splitter_len);
+
 /* Runs the whole compaction as pipelined subcompactions. options->range_* must be empty and
  * options->cuda_stream is ignored (every range gets a private stream). If
  * options->has_largest_user_key == 0 the key (Compaction::GetLargestUserKey) is read from the last
  * data block of every input on the host. outputs: max_subcompactions slots, filled in range order;
- * *num_outputs = number of ranges. err (optional) receives the message of the first failure. */
+ * *num_outputs = number of ranges. err (optional) receives the message of the first failure.
+ *
+ * options->device_memory_budget != 0 is the budget of the whole compaction (ranges in flight together):
+ *   * every range runs as a job with the budget B / max_in_flight and holds that reservation until it has run; it then
+ *     holds its measured device_bytes_peak until it is destroyed. A range starts only while the reservations of the
+ *     ranges on the device leave room for it, so the ranges' peaks at any moment sum to at most B;
+ *   * max_subcompactions == 0: as many ranges as the budget needs; the first plan gives every range about
+ *     (B / max_in_flight) / 3 bytes of input (inputs + uncompressed image), through ybgpu_plan_subcompactions;
+ *   * a range whose job fails with "device memory budget exceeded" is cut in two at a row boundary (ybgpu_split_range)
+ *     and both halves run in its place, one after the other; nothing of the failed attempt reached the caller's buffers.
+ *     A range that cannot be cut (one row needs more than the budget) fails the compaction with that message;
+ *   * outputs: *num_outputs on entry is the number of slots of `outputs` (ranges can outnumber max_subcompactions);
+ *     YBGPU_INVALID_ARGUMENT if more ranges were needed. Ranges stay in key order; ybgpu_sub_output is as without a budget.
+ *   * total->device_bytes_peak: the high-water mark of the bytes the ranges hold at once (as without a budget). */
 ybgpu_status ybgpu_compact_files(const ybgpu_job_options* options, const ybgpu_input_file* files, uint32_t num_files,
                                  uint32_t max_subcompactions, uint32_t max_in_flight,
                                  uint8_t* data_arena, uint64_t data_arena_cap, uint8_t* meta_arena, uint64_t meta_arena_cap,
                                  const volatile int32_t* shutting_down, ybgpu_sub_output* outputs, uint32_t* num_outputs,
                                  ybgpu_job_stats* total, char* err, uint64_t err_cap);
 
-/* The same pipelined compaction with ONE output table — the shape DocDB's single-level universal compaction needs
+/* The same pipelined compaction with ONE output table (device_memory_budget as for ybgpu_compact_files; every range that
+ * was cut adds a block cut at its join, like any range boundary) — the shape DocDB's single-level universal compaction needs
  * (one sorted run per compaction; db/compaction.cc:593-604 never forms subcompactions there) and the shape
  * CompactionJob::Run writes without subcompactions. The key ranges still run pipelined on private streams, but
  *   * every range's data blocks are copied device->host straight to their final position in data_out (a range's
@@ -508,6 +546,13 @@ ybgpu_status ybgpu_sst_last_key(const uint8_t* meta_file, uint64_t meta_file_len
  * CompressionType 0..7 (rocksdb/options.h:92-101). */
 ybgpu_status ybgpu_sst_check_supported(const uint8_t* meta_file, uint64_t meta_file_len, const uint8_t* data_file,
                                        uint64_t data_file_len, uint64_t counts[8]);
+
+/* What a job will need for the uncompressed image of this table (device_memory_budget's check before upload): every data
+ * block's contents + 5-byte trailer, the contents' size read from the varint32 preamble of a Snappy / LZ4 / LZ4HC block and
+ * the stored size of a raw one. A job allocates the image only when some input block is stored compressed:
+ * *compressed_blocks counts those. Host only. YBGPU_CORRUPTION: the metadata file does not parse or a handle is outside. */
+ybgpu_status ybgpu_sst_uncompressed_bytes(const uint8_t* meta_file, uint64_t meta_file_len, const uint8_t* data_file,
+                                          uint64_t data_file_len, uint64_t* image_bytes, uint64_t* compressed_blocks);
 
 /* Device-side checksum of the surviving KV stream: order-sensitive 64-bit hash over
  * (key_len, key, value_len, value) per entry, combined per entry position. Used by the parity

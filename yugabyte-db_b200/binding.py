@@ -43,6 +43,7 @@ class JobOptions(C.Structure):
         ("yield_fn", C.c_void_p), ("yield_ctx", C.c_void_p),
         ("compute_user_boundary_values", C.c_int32),
         ("output_compression", C.c_int32),
+        ("device_memory_budget", C.c_uint64),
     ]
 
 
@@ -65,7 +66,7 @@ class JobStats(C.Structure):
         "output_data_file_size", "output_meta_file_size", "smallest_seqno", "largest_seqno")] + [
         ("gpu_seconds", C.c_double), ("gpu_kernel_launches", C.c_uint32), ("h2d_bytes", C.c_uint64),
         ("d2h_bytes", C.c_uint64), ("phase_seconds", C.c_double * 8), ("phase_launches", C.c_uint32 * 8),
-                ("path_flags", C.c_uint32), ("tiles_inside_rows", C.c_uint32)]
+                ("path_flags", C.c_uint32), ("tiles_inside_rows", C.c_uint32), ("device_bytes_peak", C.c_uint64)]
 
     def as_dict(self):
         d = {n: getattr(self, n) for n, _ in self._fields_}
@@ -196,9 +197,10 @@ def make_options(device=0, bottommost=True, last_sequence=MAX_SEQUENCE, largest_
                  restart_interval=16, deviation=10, output_key_encoding=1, index_block_size=32768,
                  min_keys_per_index_block=100, verify_checksums=True, cuda_stream=None, range_lower=b"", range_upper=b"",
                  filter_policy=0, filter_block_size=65536, yield_fn=None, user_boundary_values=False,
-                 output_compression=0):
+                 output_compression=0, device_memory_budget=0):
     """ybgpu_job_options from keyword arguments; returns (options, objects to keep alive). yield_fn: a Python
-    callable() invoked at the engine's yield points (PauseIfNecessary)."""
+    callable() invoked at the engine's yield points (PauseIfNecessary). device_memory_budget: bytes of HBM the job
+    (or the whole pipelined compaction) may hold at once, 0 = unlimited."""
     L = lib()
     o = JobOptions()
     L.ybgpu_job_options_init(C.byref(o))
@@ -225,6 +227,7 @@ def make_options(device=0, bottommost=True, last_sequence=MAX_SEQUENCE, largest_
     o.range_upper, o.range_upper_len = range_upper, len(range_upper)
     o.compute_user_boundary_values = int(bool(user_boundary_values))
     o.output_compression = int(output_compression)
+    o.device_memory_budget = int(device_memory_budget)
     cb = None
     if yield_fn is not None:
         cb = YIELD_FN(lambda _ctx: yield_fn())
@@ -240,13 +243,15 @@ class GpuCompactionJob:
                  retain_delete_markers=False, other_min_ht=HT_MAX, lower=b"", upper=b"", block_size=32768,
                  restart_interval=16, deviation=10, output_key_encoding=1, index_block_size=32768,
                  min_keys_per_index_block=100, verify_checksums=True, cuda_stream=None, range_lower=b"", range_upper=b"",
-                 filter_policy=0, filter_block_size=65536, yield_fn=None, user_boundary_values=False, output_compression=0):
+                 filter_policy=0, filter_block_size=65536, yield_fn=None, user_boundary_values=False, output_compression=0,
+                 device_memory_budget=0):
         L = lib()
         o, self._keep = make_options(device, bottommost, last_sequence, largest_user_key, retention, cutoff_ht,
                                      cotables_cutoff_ht, table_ttl_ns, retain_delete_markers, other_min_ht, lower, upper,
                                      block_size, restart_interval, deviation, output_key_encoding, index_block_size,
                                      min_keys_per_index_block, verify_checksums, cuda_stream, range_lower, range_upper,
-                                     filter_policy, filter_block_size, yield_fn, user_boundary_values, output_compression)
+                                     filter_policy, filter_block_size, yield_fn, user_boundary_values, output_compression,
+                                     device_memory_budget)
         h = C.c_void_p()
         st = L.ybgpu_job_create(C.byref(o), C.byref(h))
         if st != 0:
@@ -614,6 +619,36 @@ def plan_subcompactions(ssts, max_subcompactions, docdb_keys=True):
     return [buf[i, :lens[i]].tobytes() for i in range(n.value)]
 
 
+def split_range(ssts, lower=b"", upper=b"", docdb_keys=True):
+    """ybgpu_split_range: the row-aligned splitter halving [lower, upper) of the inputs, or None when no row boundary
+    lies inside the range."""
+    L = lib()
+    L.ybgpu_split_range.argtypes = [C.c_void_p, C.c_uint32, C.c_int32, C.c_char_p, C.c_uint32, C.c_char_p, C.c_uint32, C.c_void_p,
+                                    C.POINTER(C.c_uint32)]
+    arr, keep = _input_files(ssts)
+    buf = np.zeros(256, np.uint8)
+    n = C.c_uint32()
+    st = L.ybgpu_split_range(arr, len(ssts), int(docdb_keys), lower, len(lower), upper, len(upper), buf.ctypes.data, C.byref(n))
+    if st == 1:                       # YBGPU_NOT_FOUND
+        return None
+    if st != 0:
+        raise YbGpuError(st, "split_range")
+    return buf[:n.value].tobytes()
+
+
+def sst_uncompressed_bytes(meta, data):
+    """ybgpu_sst_uncompressed_bytes: (uncompressed image bytes, blocks stored compressed) of one table, read on the host."""
+    L = lib()
+    L.ybgpu_sst_uncompressed_bytes.argtypes = [C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
+    meta = np.ascontiguousarray(meta, dtype=np.uint8)
+    data = np.ascontiguousarray(data, dtype=np.uint8)
+    img, nc = C.c_uint64(), C.c_uint64()
+    st = L.ybgpu_sst_uncompressed_bytes(meta.ctypes.data, meta.size, data.ctypes.data, data.size, C.byref(img), C.byref(nc))
+    if st != 0:
+        raise YbGpuError(st, L.ybgpu_last_error().decode())
+    return img.value, nc.value
+
+
 def sst_last_key(meta, data):
     """Last internal key of a split SST (FileMetaData::largest), read on the host."""
     L = lib()
@@ -639,10 +674,11 @@ class SubcompactionResult:
 
 
 def compact_files(ssts, max_subcompactions=8, max_in_flight=3, data_arena=None, meta_arena=None, ht_filters=None, cotable_filters=None,
-                  verify_outputs=None, **job_kwargs):
+                  verify_outputs=None, output_slots=None, **job_kwargs):
     """ybgpu_compact_files: one compaction as pipelined key-range subcompactions (one output SST per
     range, in range order). ssts: list of (meta ndarray, data ndarray) in host memory. verify_outputs (True / False):
-    ybgpu_compact_files_checked, every range's table checked on the GPU before it is copied out."""
+    ybgpu_compact_files_checked, every range's table checked on the GPU before it is copied out. With a
+    device_memory_budget, ranges may be cut further: output_slots (default 1024) bounds how many."""
     L = lib()
     L.ybgpu_compact_files.argtypes = [C.POINTER(JobOptions), C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint64,
                                       C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.POINTER(C.c_uint32), C.POINTER(JobStats),
@@ -651,12 +687,13 @@ def compact_files(ssts, max_subcompactions=8, max_in_flight=3, data_arena=None, 
     o, keep_o = make_options(**job_kwargs)
     arr, keep = _input_files(ssts, ht_filters, cotable_filters)
     in_bytes = sum(int(d.size) for _, d in ssts)
+    slots = max(1, max_subcompactions) if not o.device_memory_budget else (output_slots or 1024)
     if data_arena is None:
-        data_arena = np.empty(in_bytes + (in_bytes >> 4) + (1 << 20) + 4096 * max_subcompactions, np.uint8)
+        data_arena = np.empty(in_bytes + (in_bytes >> 4) + (1 << 20) + 4096 * slots, np.uint8)
     if meta_arena is None:
-        meta_arena = np.empty((in_bytes >> 5) + (4 << 20) + 4096 * max_subcompactions, np.uint8)
-    outs = (SubOutput * max(1, max_subcompactions))()
-    n = C.c_uint32()
+        meta_arena = np.empty((in_bytes >> 5) + (4 << 20) + 4096 * slots, np.uint8)
+    outs = (SubOutput * slots)()
+    n = C.c_uint32(slots)
     total = JobStats()
     err = C.create_string_buffer(512)
     args = (C.byref(o), arr, len(ssts), max_subcompactions, max_in_flight, data_arena.ctypes.data, data_arena.size,

@@ -36,6 +36,8 @@ struct ybgpu_job {
 
 static thread_local std::string g_last_error;
 
+void ybgpu::JoinMemGroup(ybgpu_job* job, MemGroup* group) { job->engine->JoinMemGroup(group); }
+
 static ybgpu_status JobFail(ybgpu_job* j, ybgpu_status s, const std::string& msg) {
   j->error = msg;
   return s;
@@ -509,6 +511,20 @@ ybgpu_status ybgpu_sst_check_supported(const uint8_t* meta, uint64_t meta_len, c
     g_last_error = std::to_string(lz4_unfit) + " data blocks labelled LZ4 do not start with an LZ4 length preamble the engine decodes";
     return YBGPU_NOT_SUPPORTED;
   }
+  return YBGPU_OK;
+}
+
+ybgpu_status ybgpu_sst_uncompressed_bytes(const uint8_t* meta, uint64_t meta_len, const uint8_t* data, uint64_t data_len,
+                                         uint64_t* image_bytes, uint64_t* compressed_blocks) {
+  if (!meta || (!data && data_len) || !image_bytes || !compressed_blocks) { g_last_error = "null argument"; return YBGPU_INVALID_ARGUMENT; }
+  ybgpu::host::SstMeta m;
+  std::string err = ybgpu::host::ParseSplitSstMeta(meta, meta_len, &m);
+  if (!err.empty()) { g_last_error = err; return YBGPU_CORRUPTION; }
+  for (const ybgpu::host::Handle& h : m.data_blocks)
+    if (h.offset > data_len || h.size > data_len - h.offset || data_len - h.offset - h.size < 5) {
+      g_last_error = "a data block handle points outside the data file"; return YBGPU_CORRUPTION;
+    }
+  *image_bytes = ybgpu::host::UncompressedImageBytes(data, m.data_blocks.data(), m.data_blocks.size(), compressed_blocks);
   return YBGPU_OK;
 }
 

@@ -317,6 +317,10 @@ class GpuCompactionJob {
     // compaction_job.cc:409-519) that run pipelined on private streams, one output file per range.
     uint32_t max_subcompactions = 1;
     uint32_t subcompactions_in_flight = 3;
+    // Bytes of HBM the job (with max_subcompactions > 1: the whole pipelined compaction) may hold at once; 0 = unlimited.
+    // A job that cannot fit is refused before upload (NotSupported) or fails when it would pass it (RuntimeError); the
+    // pipelined compaction cuts a range that needs more into two at a row boundary and runs the halves instead.
+    uint64_t device_memory_budget = 0;
     // Yield point, e.g. [](void* s) { static_cast<yb::PriorityThreadPoolSuspender*>(s)->PauseIfNecessary(); }
     // (util/file_reader_writer.cc:343): called between kernel phases and between subcompaction ranges.
     void (*yield_fn)(void*) = nullptr;
@@ -357,6 +361,7 @@ class GpuCompactionJob {
     o.min_keys_per_index_block = p_.min_keys_per_index_block; o.verify_checksums = p_.verify_checksums;
     o.output_key_encoding = p_.output_key_encoding; o.filter_policy = p_.filter_policy; o.filter_block_size = p_.filter_block_size;
     o.output_compression = p_.output_compression;
+    o.device_memory_budget = p_.device_memory_budget;
     o.yield_fn = p_.yield_fn; o.yield_ctx = p_.yield_ctx;
     o.compute_user_boundary_values = p_.retention.CouldChangeKeyRange() && p_.max_subcompactions <= 1;
     options_ = o;
@@ -424,10 +429,12 @@ class GpuCompactionJob {
     }
     // the output of a compaction is never larger than its input plus per-file metadata
     std::string data_arena, meta_arena;
-    data_arena.resize(in_bytes + in_bytes / 16 + (1u << 20) + 4096ull * p_.max_subcompactions);
-    meta_arena.resize(in_bytes / 32 + (4u << 20) + 4096ull * p_.max_subcompactions);
-    std::vector<ybgpu_sub_output> outs(p_.max_subcompactions);
-    uint32_t n = 0;
+    // under a budget a range may be cut again: room for more outputs than planned ranges
+    const uint32_t slots = p_.device_memory_budget ? std::max<uint32_t>(1024, p_.max_subcompactions) : p_.max_subcompactions;
+    data_arena.resize(in_bytes + in_bytes / 16 + (1u << 20) + 4096ull * slots);
+    meta_arena.resize(in_bytes / 32 + (4u << 20) + 4096ull * slots);
+    std::vector<ybgpu_sub_output> outs(slots);
+    uint32_t n = slots;
     char err[512] = {0};
     ybgpu_status s = ybgpu_compact_files_checked(&o, files.data(), static_cast<uint32_t>(files.size()), p_.max_subcompactions,
                                                  p_.subcompactions_in_flight, reinterpret_cast<uint8_t*>(&data_arena[0]), data_arena.size(),

@@ -31,7 +31,7 @@ namespace ybgpu {
   do {                                                                                      \
     cudaError_t _e = (expr);                                                                \
     if (_e != cudaSuccess) {                                                                \
-      return Fail(YBGPU_RUNTIME_ERROR, std::string(#expr) + ": " + cudaGetErrorString(_e)); \
+      return FailCuda(#expr, _e);                                                           \
     }                                                                                       \
   } while (0)
 
@@ -1469,6 +1469,45 @@ static ybgpu_status DevErrorStatus(int e) {
   }
 }
 
+// Every device allocation and free of a job goes through here: the job's own buffers, the early frees after the output
+// gather and the output check's temporaries. It keeps the live blocks, the requested bytes in use (the engine's 32-byte
+// pads included; the pool's rounding to its own granularity is not counted), their high-water mark and the job's
+// device_memory_budget (0 = none: then nothing is checked and allocation is a plain cudaMallocAsync).
+struct JobMemory {
+  std::vector<std::pair<void*, size_t>> live;
+  uint64_t in_use = 0, peak = 0, budget = 0;
+  MemGroup* group = nullptr;           // the jobs whose bytes live at once are counted together (pipelined ranges)
+  uint64_t refused = 0;                // size of the request the budget just refused (0 = none)
+  static size_t Padded(size_t bytes) { return std::max<size_t>(bytes, 16) + 32; }
+  bool Fits(uint64_t more) const { return !budget || (more <= budget && in_use <= budget - more); }
+  cudaError_t Alloc(void** p, size_t bytes, cudaStream_t s) {
+    if (!Fits(bytes)) { refused = bytes; return cudaErrorMemoryAllocation; }
+    cudaError_t e = cudaMallocAsync(p, bytes, s);
+    if (e != cudaSuccess) return e;
+    live.emplace_back(*p, bytes);
+    in_use += bytes;
+    peak = std::max(peak, in_use);
+    if (group) group->Change(static_cast<int64_t>(bytes));
+    return cudaSuccess;
+  }
+  cudaError_t Free(void* p, cudaStream_t s) {
+    for (size_t i = live.size(); i-- > 0;)
+      if (live[i].first == p) {
+        in_use -= live[i].second;
+        if (group) group->Change(-static_cast<int64_t>(live[i].second));
+        live.erase(live.begin() + i);
+        return cudaFreeAsync(p, s);
+      }
+    return cudaSuccess;
+  }
+  void FreeAll(cudaStream_t s) {
+    for (auto& a : live) cudaFreeAsync(a.first, s);
+    live.clear();
+    if (group) group->Change(-static_cast<int64_t>(in_use));
+    in_use = 0;
+  }
+};
+
 struct Engine::Impl {
   cudaStream_t stream = nullptr;
   bool owns_stream = false;            // cuda_stream == YBGPU_STREAM_PRIVATE: created in Init, destroyed with the job
@@ -1487,7 +1526,8 @@ struct Engine::Impl {
   bool enc_timed = false;
   cudaEvent_t snap_ev[4] = {};         // around the output block compressor (Snappy or LZ4) and the gather of the stored blocks
   bool snap_timed = false;
-  std::vector<void*> allocs;
+  JobMemory mem;
+  uint64_t image_bytes = 0, compressed_blocks = 0;   // uncompressed image the inputs added so far will need (host-known)
   JobDev* dJ = nullptr;
   JobParams* dP = nullptr;
   RunView* dRuns = nullptr;
@@ -1631,6 +1671,7 @@ Engine::Engine(const ybgpu_job_options& o) : opt_(o), impl_(new Impl) {
   opt_.range_lower = nullptr; opt_.range_upper = nullptr;
   opt_.largest_user_key = nullptr; opt_.key_bounds_lower = nullptr; opt_.key_bounds_upper = nullptr;
   memset(&stats_, 0, sizeof(stats_));
+  impl_->mem.budget = o.device_memory_budget;
 }
 
 Engine::~Engine() {
@@ -1639,7 +1680,7 @@ Engine::~Engine() {
     if (impl_->copy_pending) cudaStreamSynchronize(impl_->copy_stream);   // before the output buffer returns to the pool
     // a job abandoned before Run() may still have input DMAs queued that read the caller's buffers
     if (!ran_ && !impl_->runs.empty()) cudaStreamSynchronize(impl_->stream);
-    for (void* p : impl_->allocs) cudaFreeAsync(p, impl_->stream);
+    impl_->mem.FreeAll(impl_->stream);
     if (impl_->ev0) cudaEventDestroy(impl_->ev0);
     if (impl_->ev1) cudaEventDestroy(impl_->ev1);
     if (impl_->copy_stream) cudaStreamDestroy(impl_->copy_stream);
@@ -1660,14 +1701,47 @@ Engine::~Engine() {
 
 ybgpu_status Engine::Fail(ybgpu_status s, const std::string& msg) { error_ = msg; return s; }
 
+static std::string BudgetMessage(uint64_t need, uint64_t in_use, uint64_t budget) {
+  return std::string(kBudgetExceeded) + ": need " + std::to_string(need) + ", in use " + std::to_string(in_use) + ", budget " +
+         std::to_string(budget);
+}
+
+ybgpu_status Engine::FailCuda(const char* expr, int e) {
+  JobMemory& M = impl_->mem;
+  if (M.refused) {
+    const uint64_t need = M.refused;
+    M.refused = 0;
+    cudaStreamSynchronize(impl_->stream);                 // nothing the failed job queued is still running when it returns
+    return Fail(YBGPU_RUNTIME_ERROR, BudgetMessage(need, M.in_use, M.budget));
+  }
+  return Fail(YBGPU_RUNTIME_ERROR, std::string(expr) + ": " + cudaGetErrorString(static_cast<cudaError_t>(e)));
+}
+
+// Host-known bytes (`more` beyond what the job holds) checked against the budget before anything is uploaded.
+ybgpu_status Engine::CheckBudgetBeforeUpload(uint64_t more) {
+  const JobMemory& M = impl_->mem;
+  if (M.Fits(more)) return YBGPU_OK;
+  return Fail(YBGPU_NOT_SUPPORTED, BudgetMessage(more, M.in_use, M.budget) + " (inputs and their uncompressed image, before upload)");
+}
+
+void Engine::JoinMemGroup(MemGroup* group) {
+  impl_->mem.group = group;
+  group->Change(static_cast<int64_t>(impl_->mem.in_use));
+}
+
+ybgpu_job_stats& Engine::stats() {
+  stats_.device_bytes_peak = impl_->mem.peak;
+  return stats_;
+}
+
 // Stream-ordered allocation from the device's default memory pool (release threshold raised to
 // "never" in Init), so steady-state jobs reuse HBM instead of paying cudaMalloc/cudaFree.
 static thread_local cudaStream_t g_alloc_stream = nullptr;
 template <typename T>
-static cudaError_t DevAlloc(std::vector<void*>* allocs, T** out, size_t count) {
+static cudaError_t DevAlloc(JobMemory* mem, T** out, size_t count) {
   void* p = nullptr;
-  cudaError_t e = cudaMallocAsync(&p, std::max<size_t>(count * sizeof(T), 16) + 32, g_alloc_stream);
-  if (e == cudaSuccess) { allocs->push_back(p); *out = reinterpret_cast<T*>(p); }
+  cudaError_t e = mem->Alloc(&p, JobMemory::Padded(count * sizeof(T)), g_alloc_stream);
+  if (e == cudaSuccess) *out = reinterpret_cast<T*>(p);
   return e;
 }
 
@@ -1727,9 +1801,9 @@ ybgpu_status Engine::Init() {
   CUDA_TRY(cudaEventCreate(&impl_->ev1));
   for (auto& e : impl_->phase_ev) CUDA_TRY(cudaEventCreate(&e));
   for (auto& e : impl_->enc_ev) CUDA_TRY(cudaEventCreate(&e));
-  CUDA_TRY(DevAlloc(&impl_->allocs, &impl_->dJ, 1));
-  CUDA_TRY(DevAlloc(&impl_->allocs, &impl_->dP, 1));
-  CUDA_TRY(DevAlloc(&impl_->allocs, &impl_->dRuns, MAX_RUNS));
+  CUDA_TRY(DevAlloc(&impl_->mem, &impl_->dJ, 1));
+  CUDA_TRY(DevAlloc(&impl_->mem, &impl_->dP, 1));
+  CUDA_TRY(DevAlloc(&impl_->mem, &impl_->dRuns, MAX_RUNS));
   return YBGPU_OK;
 }
 
@@ -1749,12 +1823,23 @@ ybgpu_status Engine::AddInput(const uint8_t* data, uint64_t len, const ybgpu_blo
       return Fail(YBGPU_CORRUPTION, "block handle outside the data file");
     if (handles[i].size >= (1ull << 31)) return Fail(YBGPU_NOT_SUPPORTED, "data block too large");
   }
+  if (impl_->mem.budget) {
+    // this input's device copy and handle arrays, and — once any input block is stored compressed — the uncompressed image
+    // of every input (a file already in device memory is not read on the host: its image is not known before run)
+    uint64_t comp = 0;
+    const uint64_t img = on_device ? 0 : host::UncompressedImageBytes(data, handles, nh, &comp);
+    uint64_t more = (on_device ? 0 : JobMemory::Padded(len + 64)) + JobMemory::Padded(nh * 8) + JobMemory::Padded(nh * 4) +
+                    JobMemory::Padded((nh + 1) * 4);
+    if (impl_->compressed_blocks + comp) more += JobMemory::Padded(impl_->image_bytes + img + 96);
+    if (ybgpu_status s = CheckBudgetBeforeUpload(more)) return s;
+    impl_->image_bytes += img; impl_->compressed_blocks += comp;
+  }
   RunView rv{};
   if (on_device) {
     rv.data = data;
   } else {
     uint8_t* d = nullptr;
-    CUDA_TRY(DevAlloc(&impl_->allocs, &d, len + 64));
+    CUDA_TRY(DevAlloc(&impl_->mem, &d, len + 64));
     // 16 bytes of zero padding on both sides so word-granular copies may over-read
     CUDA_TRY(cudaMemsetAsync(d, 0, 16, impl_->stream));
     CUDA_TRY(ChunkedCopyAsync(d + 16, data, len, cudaMemcpyHostToDevice, impl_->stream));
@@ -1768,8 +1853,8 @@ ybgpu_status Engine::AddInput(const uint8_t* data, uint64_t len, const ybgpu_blo
   std::vector<uint64_t>& off = impl_->keep_off.back(); std::vector<uint32_t>& sz = impl_->keep_sz.back();
   for (uint64_t i = 0; i < nh; i++) { off[i] = handles[i].offset; sz[i] = static_cast<uint32_t>(handles[i].size); }
   uint64_t* doff = nullptr; uint32_t* dsz = nullptr; uint32_t* dcnt = nullptr;
-  CUDA_TRY(DevAlloc(&impl_->allocs, &doff, nh)); CUDA_TRY(DevAlloc(&impl_->allocs, &dsz, nh));
-  CUDA_TRY(DevAlloc(&impl_->allocs, &dcnt, nh + 1));
+  CUDA_TRY(DevAlloc(&impl_->mem, &doff, nh)); CUDA_TRY(DevAlloc(&impl_->mem, &dsz, nh));
+  CUDA_TRY(DevAlloc(&impl_->mem, &dcnt, nh + 1));
   CUDA_TRY(cudaMemcpyAsync(doff, off.data(), nh * 8, cudaMemcpyHostToDevice, impl_->stream));
   CUDA_TRY(cudaMemcpyAsync(dsz, sz.data(), nh * 4, cudaMemcpyHostToDevice, impl_->stream));
   rv.blk_off = doff; rv.blk_size = dsz; rv.blk_count = dcnt; rv.nb = static_cast<uint32_t>(nh);
@@ -1806,10 +1891,15 @@ ybgpu_status Engine::AddInputKv(const uint8_t* keys, const uint64_t* key_offsets
     if (key_offsets[i + 1] < key_offsets[i] + 8 || value_offsets[i + 1] < value_offsets[i]) return Fail(YBGPU_INVALID_ARGUMENT, "bad key / value offsets");
     max_klen = std::max<uint32_t>(max_klen, static_cast<uint32_t>(std::min<uint64_t>(key_offsets[i + 1] - key_offsets[i], 0xffffffffu)));
   }
+  if (I.mem.budget) {
+    const uint64_t more = JobMemory::Padded(kbytes + 16) + JobMemory::Padded(vbytes + 64) + 2 * JobMemory::Padded((n + 1) * 8) +
+                          JobMemory::Padded(4);
+    if (ybgpu_status s = CheckBudgetBeforeUpload(more)) return s;
+  }
   uint8_t* dk = nullptr; uint8_t* dv = nullptr; unsigned long long* dko = nullptr; unsigned long long* dvo = nullptr; uint32_t* dcnt = nullptr;
-  CUDA_TRY(DevAlloc(&I.allocs, &dk, kbytes + 16));
-  CUDA_TRY(DevAlloc(&I.allocs, &dv, vbytes + 64));
-  CUDA_TRY(DevAlloc(&I.allocs, &dko, n + 1)); CUDA_TRY(DevAlloc(&I.allocs, &dvo, n + 1)); CUDA_TRY(DevAlloc(&I.allocs, &dcnt, 1));
+  CUDA_TRY(DevAlloc(&I.mem, &dk, kbytes + 16));
+  CUDA_TRY(DevAlloc(&I.mem, &dv, vbytes + 64));
+  CUDA_TRY(DevAlloc(&I.mem, &dko, n + 1)); CUDA_TRY(DevAlloc(&I.mem, &dvo, n + 1)); CUDA_TRY(DevAlloc(&I.mem, &dcnt, 1));
   CUDA_TRY(cudaMemsetAsync(dv, 0, 16, I.stream));
   if (kbytes) CUDA_TRY(ChunkedCopyAsync(dk, keys, kbytes, cudaMemcpyHostToDevice, I.stream));
   if (vbytes) CUDA_TRY(ChunkedCopyAsync(dv + 16, values, vbytes, cudaMemcpyHostToDevice, I.stream));
@@ -1950,6 +2040,8 @@ static cudaError_t EnsureDeviceTables(int device, cudaStream_t stream, int* sms)
 ybgpu_status Engine::Run(const volatile int32_t* shutting_down) {
   if (ran_) return Fail(YBGPU_ILLEGAL_STATE, "job already ran");
   Impl& I = *impl_;
+  if (I.compressed_blocks)                                // counted only under a budget: the uncompressed image comes first
+    if (ybgpu_status s = CheckBudgetBeforeUpload(JobMemory::Padded(I.image_bytes + 96))) return s;
   const bool trace = getenv("YBGPU_TRACE") != nullptr;
   auto t_prev = std::chrono::steady_clock::now();
   CUDA_TRY(cudaSetDevice(opt_.device));
@@ -1989,16 +2081,16 @@ ybgpu_status Engine::Run(const volatile int32_t* shutting_down) {
   // key records) when every input is shared-prefix encoded; otherwise, or when the fused kernel meets something
   // it does not take, the general kernels: k_crc_blocks (verify), k_prepass, k_decode_all, k_value_crc.
   uint32_t* d_totals = nullptr;
-  CUDA_TRY(DevAlloc(&I.allocs, &d_totals, static_cast<size_t>(k) + 1));
+  CUDA_TRY(DevAlloc(&I.mem, &d_totals, static_cast<size_t>(k) + 1));
   std::vector<uint32_t> blk_base(k + 1, 0);
   for (int r = 0; r < k; r++) blk_base[r + 1] = blk_base[r] + I.runs[r].nb;
   uint32_t* d_blk_base = nullptr;
-  CUDA_TRY(DevAlloc(&I.allocs, &d_blk_base, static_cast<size_t>(k) + 1));
+  CUDA_TRY(DevAlloc(&I.mem, &d_blk_base, static_cast<size_t>(k) + 1));
   for (int r = 0; r < k; r++) {
     const size_t n = I.cf_oids[r].size();
     if (!n || I.runs[r].cf_n) continue;
     uint32_t* d_oid = nullptr; uint64_t* d_ht = nullptr;
-    CUDA_TRY(DevAlloc(&I.allocs, &d_oid, n)); CUDA_TRY(DevAlloc(&I.allocs, &d_ht, n));
+    CUDA_TRY(DevAlloc(&I.mem, &d_oid, n)); CUDA_TRY(DevAlloc(&I.mem, &d_ht, n));
     if (ybgpu_status us = UploadSmall(d_oid, I.cf_oids[r].data(), 4 * n)) return us;
     if (ybgpu_status us = UploadSmall(d_ht, I.cf_hts[r].data(), 8 * n)) return us;
     I.runs[r].cf_oid = d_oid; I.runs[r].cf_ht = d_ht; I.runs[r].cf_n = static_cast<uint32_t>(n);
@@ -2011,7 +2103,7 @@ ybgpu_status Engine::Run(const volatile int32_t* shutting_down) {
     RangeDev hr{};
     hr.lower_len = static_cast<uint32_t>(range_lower_.size()); memcpy(hr.lower, range_lower_.data(), range_lower_.size());
     hr.upper_len = static_cast<uint32_t>(range_upper_.size()); memcpy(hr.upper, range_upper_.data(), range_upper_.size());
-    CUDA_TRY(DevAlloc(&I.allocs, &d_range, 1));
+    CUDA_TRY(DevAlloc(&I.mem, &d_range, 1));
     if (ybgpu_status us = UploadSmall(d_range, &hr, sizeof(hr))) return us;
   }
   uint64_t N = 0;
@@ -2036,9 +2128,9 @@ ybgpu_status Engine::Run(const volatile int32_t* shutting_down) {
     CUDA_TRY(end_phase());
     for (int r = 0; r < k; r++) {
       RunView& rv = I.runs[r];
-      CUDA_TRY(DevAlloc(&I.allocs, &rv.rec, static_cast<size_t>(rv.n_entries) * Sfinal + 16));
-      CUDA_TRY(DevAlloc(&I.allocs, &rv.val_off, static_cast<size_t>(rv.n_entries) + 1));
-      CUDA_TRY(DevAlloc(&I.allocs, &rv.val_crc, static_cast<size_t>(rv.n_entries) + 1));
+      CUDA_TRY(DevAlloc(&I.mem, &rv.rec, static_cast<size_t>(rv.n_entries) * Sfinal + 16));
+      CUDA_TRY(DevAlloc(&I.mem, &rv.val_off, static_cast<size_t>(rv.n_entries) + 1));
+      CUDA_TRY(DevAlloc(&I.mem, &rv.val_crc, static_cast<size_t>(rv.n_entries) + 1));
       if (rv.n_entries) {
         k_records_from_kv<<<GridFor(rv.n_entries, 256, sms), 256, 0, I.stream>>>(I.kv[r].keys, I.kv[r].koff, I.kv[r].voff, rv.data, rv.n_entries, Sfinal,
                                                                              rv.rec, rv.val_off, I.dJ);
@@ -2077,10 +2169,10 @@ ybgpu_status Engine::Run(const volatile int32_t* shutting_down) {
       }
       SnapView sv{};
       sv.runs = I.dRuns; sv.blk_base = d_blk_base; sv.k = k;
-      CUDA_TRY(DevAlloc(&I.allocs, &sv.out_off, static_cast<size_t>(blk_base[k]) + 1));
-      CUDA_TRY(DevAlloc(&I.allocs, &sv.usize, static_cast<size_t>(blk_base[k])));
+      CUDA_TRY(DevAlloc(&I.mem, &sv.out_off, static_cast<size_t>(blk_base[k]) + 1));
+      CUDA_TRY(DevAlloc(&I.mem, &sv.usize, static_cast<size_t>(blk_base[k])));
       unsigned long long* d_img = nullptr;
-      CUDA_TRY(DevAlloc(&I.allocs, &d_img, 1));
+      CUDA_TRY(DevAlloc(&I.mem, &d_img, 1));
       k_snappy_sizes<<<GridFor(blk_base[k], 256, sms), 256, 0, I.stream>>>(sv, I.dJ);
       k_scan_u64_single<<<1, 1024, 0, I.stream>>>(sv.out_off, blk_base[k], d_img);
       launches += 2;
@@ -2089,7 +2181,7 @@ ybgpu_status Engine::Run(const volatile int32_t* shutting_down) {
       unsigned long long img_bytes = 0;
       if (ybgpu_status s = ReadSmall(&img_bytes, d_img, 8)) return s;
       uint8_t* img = nullptr;
-      CUDA_TRY(DevAlloc(&I.allocs, &img, img_bytes + 96));
+      CUDA_TRY(DevAlloc(&I.mem, &img, img_bytes + 96));
       CUDA_TRY(cudaMemsetAsync(img, 0, 16, I.stream));
       CUDA_TRY(cudaMemsetAsync(img + 16 + img_bytes, 0, 64, I.stream));
       sv.out = img + 16;
@@ -2133,15 +2225,15 @@ ybgpu_status Engine::Run(const volatile int32_t* shutting_down) {
     const uint32_t sample_max = std::max<uint32_t>(I.hJ.max_ikey_len, 8);
     Sfinal = std::min(S_widest, std::max(32, static_cast<int>(((sample_max - 8 + 16) + 15) & ~15u)));
     IngestView iv{};
-    CUDA_TRY(DevAlloc(&I.allocs, &iv.ticket, 1));
+    CUDA_TRY(DevAlloc(&I.mem, &iv.ticket, 1));
     CUDA_TRY(cudaFuncSetAttribute(k_ingest, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(ING_SMEM)));
     for (int attempt = 0; attempt < 2; attempt++) {
       for (int r = 0; r < k; r++) {
         RunView& rv = I.runs[r];
-        CUDA_TRY(DevAlloc(&I.allocs, &rv.rec, static_cast<size_t>(cap[r]) * Sfinal + 16));
+        CUDA_TRY(DevAlloc(&I.mem, &rv.rec, static_cast<size_t>(cap[r]) * Sfinal + 16));
         if (attempt == 0) {
-          CUDA_TRY(DevAlloc(&I.allocs, &rv.val_off, static_cast<size_t>(cap[r]) + 1));
-          CUDA_TRY(DevAlloc(&I.allocs, &rv.val_crc, static_cast<size_t>(cap[r]) + 1));
+          CUDA_TRY(DevAlloc(&I.mem, &rv.val_off, static_cast<size_t>(cap[r]) + 1));
+          CUDA_TRY(DevAlloc(&I.mem, &rv.val_crc, static_cast<size_t>(cap[r]) + 1));
         }
       }
       if (ybgpu_status us = UploadSmall(I.dRuns, I.runs.data(), sizeof(RunView) * k)) return us;
@@ -2217,15 +2309,15 @@ ybgpu_status Engine::Run(const volatile int32_t* shutting_down) {
     std::vector<uint32_t> group_base(k + 1, 0);
     for (int r = 0; r < k; r++) {
       RunView& rv = I.runs[r];
-      CUDA_TRY(DevAlloc(&I.allocs, &rv.rec, static_cast<size_t>(rv.n_entries) * Sfinal + 16));
-      CUDA_TRY(DevAlloc(&I.allocs, &rv.val_off, static_cast<size_t>(rv.n_entries) + 1));
-      CUDA_TRY(DevAlloc(&I.allocs, &rv.val_crc, static_cast<size_t>(rv.n_entries) + 1));
+      CUDA_TRY(DevAlloc(&I.mem, &rv.rec, static_cast<size_t>(rv.n_entries) * Sfinal + 16));
+      CUDA_TRY(DevAlloc(&I.mem, &rv.val_off, static_cast<size_t>(rv.n_entries) + 1));
+      CUDA_TRY(DevAlloc(&I.mem, &rv.val_crc, static_cast<size_t>(rv.n_entries) + 1));
       group_base[r + 1] = group_base[r] + (rv.nb + DEC_WB - 1) / DEC_WB;
     }
     if (ybgpu_status us = UploadSmall(I.dRuns, I.runs.data(), sizeof(RunView) * k)) return us;
     if (group_base[k]) {
       uint32_t* d_group_base = nullptr;
-      CUDA_TRY(DevAlloc(&I.allocs, &d_group_base, k + 1));
+      CUDA_TRY(DevAlloc(&I.mem, &d_group_base, k + 1));
       if (ybgpu_status us = UploadSmall(d_group_base, group_base.data(), 4 * (k + 1))) return us;
       const int grid = GridFor(static_cast<uint64_t>(group_base[k]) * 32, 128, sms);
       // fast path: shared-prefix inputs, internal keys of at most 64 bytes, no HybridTime filter / key range
@@ -2322,12 +2414,12 @@ ybgpu_status Engine::Run(const volatile int32_t* shutting_down) {
     const uint32_t n_buckets = static_cast<uint32_t>(N / hp.H) + 2;
     PartView pv{};
     uint32_t* d_sample_base = nullptr;
-    CUDA_TRY(DevAlloc(&I.allocs, &d_sample_base, k + 1));
-    CUDA_TRY(DevAlloc(&I.allocs, &pv.pos, static_cast<size_t>(n_samples) * k));
-    CUDA_TRY(DevAlloc(&I.allocs, &pv.smode, n_samples));
-    CUDA_TRY(DevAlloc(&I.allocs, &pv.bucket_min, n_buckets));
-    CUDA_TRY(DevAlloc(&I.allocs, &d_tile_lo, static_cast<size_t>(n_buckets + 1) * k));
-    CUDA_TRY(DevAlloc(&I.allocs, &d_tile_rank, n_buckets + 1));
+    CUDA_TRY(DevAlloc(&I.mem, &d_sample_base, k + 1));
+    CUDA_TRY(DevAlloc(&I.mem, &pv.pos, static_cast<size_t>(n_samples) * k));
+    CUDA_TRY(DevAlloc(&I.mem, &pv.smode, n_samples));
+    CUDA_TRY(DevAlloc(&I.mem, &pv.bucket_min, n_buckets));
+    CUDA_TRY(DevAlloc(&I.mem, &d_tile_lo, static_cast<size_t>(n_buckets + 1) * k));
+    CUDA_TRY(DevAlloc(&I.mem, &d_tile_rank, n_buckets + 1));
     if (ybgpu_status us = UploadSmall(d_sample_base, sample_base.data(), 4 * (k + 1))) return us;
     CUDA_TRY(cudaMemsetAsync(pv.bucket_min, 0xff, static_cast<size_t>(n_buckets) * 8, I.stream));
     pv.runs = I.dRuns; pv.sample_base = d_sample_base; pv.n_samples = n_samples; pv.n_buckets = n_buckets;
@@ -2337,7 +2429,7 @@ ybgpu_status Engine::Run(const volatile int32_t* shutting_down) {
     {
       const uint32_t tchunks = (n_buckets + TILE_CHUNK - 1) / TILE_CHUNK;
       uint32_t* d_tpart = nullptr; uint32_t* d_ttotal = nullptr;
-      CUDA_TRY(DevAlloc(&I.allocs, &d_tpart, tchunks + 1)); CUDA_TRY(DevAlloc(&I.allocs, &d_ttotal, 1));
+      CUDA_TRY(DevAlloc(&I.mem, &d_tpart, tchunks + 1)); CUDA_TRY(DevAlloc(&I.mem, &d_ttotal, 1));
       k_bucket_counts<<<tchunks, 256, 0, I.stream>>>(pv, d_tpart);
       k_scan_u32_single<<<1, 1024, 0, I.stream>>>(d_tpart, tchunks, d_ttotal);
       k_build_tiles<<<tchunks, 256, 0, I.stream>>>(pv, I.dP, d_tpart, d_ttotal, d_tile_lo, d_tile_rank, I.dJ);
@@ -2361,16 +2453,16 @@ ybgpu_status Engine::Run(const volatile int32_t* shutting_down) {
   // ---- K3: merge + filter
   Desc* d_desc = nullptr; ValueRewrite* d_rw = nullptr;
   const uint32_t rewrite_cap = static_cast<uint32_t>(std::min<uint64_t>(N, 1u << 26));
-  CUDA_TRY(DevAlloc(&I.allocs, &d_desc, N));
-  CUDA_TRY(DevAlloc(&I.allocs, &d_rw, rewrite_cap));
+  CUDA_TRY(DevAlloc(&I.mem, &d_desc, N));
+  CUDA_TRY(DevAlloc(&I.mem, &d_rw, rewrite_cap));
   MergeView mv{};
   mv.runs = I.dRuns; mv.tile_lo = d_tile_lo; mv.tile_rank = d_tile_rank; mv.desc = d_desc;
   mv.rewrites = d_rw; mv.rewrite_cap = rewrite_cap; mv.n_tiles = n_tiles;
   uint16_t* d_fk16 = nullptr;
-  if (opt_.filter_policy != YBGPU_FILTER_NONE && getenv("YBGPU_NO_FK16") == nullptr) CUDA_TRY(DevAlloc(&I.allocs, &d_fk16, N));
+  if (opt_.filter_policy != YBGPU_FILTER_NONE && getenv("YBGPU_NO_FK16") == nullptr) CUDA_TRY(DevAlloc(&I.mem, &d_fk16, N));
   mv.fk16 = d_fk16;
   uint32_t* d_fkh = nullptr;
-  if (d_fk16) CUDA_TRY(DevAlloc(&I.allocs, &d_fkh, N));
+  if (d_fk16) CUDA_TRY(DevAlloc(&I.mem, &d_fkh, N));
   mv.fkh = d_fkh;
   mv.S = Sfinal; mv.k = k; mv.cap = cap;
   const size_t smem = tile_layout::bytes(Sfinal, cap);
@@ -2387,7 +2479,7 @@ ybgpu_status Engine::Run(const volatile int32_t* shutting_down) {
   I.n_out = I.hJ.n_kept; I.out_key_bytes = I.hJ.out_key_bytes; I.out_val_bytes = I.hJ.out_val_bytes;
   const uint32_t n_chunks = static_cast<uint32_t>((N + EMIT_CHUNK - 1) / EMIT_CHUNK);
   Sums3* d_partial = nullptr;
-  CUDA_TRY(DevAlloc(&I.allocs, &d_partial, n_chunks + 1));
+  CUDA_TRY(DevAlloc(&I.mem, &d_partial, n_chunks + 1));
   I.d_desc = d_desc; I.d_partial = d_partial; I.d_rw = d_rw; I.N = N; I.S = Sfinal; I.n_chunks = n_chunks;
   // the chunk sums place survivors among dropped entries: k_compact_desc needs them now, k_emit when the KV stream is asked for
   I.partial_ready = false;
@@ -2403,7 +2495,7 @@ ybgpu_status Engine::Run(const volatile int32_t* shutting_down) {
     if (static_cast<uint64_t>(n) == N) {
       I.d_kept = d_desc;                                  // nothing was dropped: the merged-order list IS the survivor list
     } else {
-      CUDA_TRY(DevAlloc(&I.allocs, &I.d_kept, n));
+      CUDA_TRY(DevAlloc(&I.mem, &I.d_kept, n));
       k_compact_desc<<<n_chunks, EMIT_THREADS, 0, I.stream>>>(d_desc, N, d_partial, I.d_kept);
     }
     EncView& E = I.enc;
@@ -2415,17 +2507,17 @@ ybgpu_status Engine::Run(const volatile int32_t* shutting_down) {
       const double avg = static_cast<double>(I.out_key_bytes + I.out_val_bytes) / n + 3.0;
       E.guess = static_cast<uint32_t>(std::max(1.0, 0.85 * opt_.block_size / avg));
     }
-    CUDA_TRY(DevAlloc(&I.allocs, &E.nr, n)); CUDA_TRY(DevAlloc(&I.allocs, &E.shared, n)); CUDA_TRY(DevAlloc(&I.allocs, &E.D, n));
-    CUDA_TRY(DevAlloc(&I.allocs, &E.P, static_cast<size_t>(n) + 1)); CUDA_TRY(DevAlloc(&I.allocs, &E.QQ, n));
-    CUDA_TRY(DevAlloc(&I.allocs, &E.next, n)); CUDA_TRY(DevAlloc(&I.allocs, &E.exit1, n));
+    CUDA_TRY(DevAlloc(&I.mem, &E.nr, n)); CUDA_TRY(DevAlloc(&I.mem, &E.shared, n)); CUDA_TRY(DevAlloc(&I.mem, &E.D, n));
+    CUDA_TRY(DevAlloc(&I.mem, &E.P, static_cast<size_t>(n) + 1)); CUDA_TRY(DevAlloc(&I.mem, &E.QQ, n));
+    CUDA_TRY(DevAlloc(&I.mem, &E.next, n)); CUDA_TRY(DevAlloc(&I.mem, &E.exit1, n));
     E.fk_len = nullptr; E.fk_src = nullptr; E.fkh_src = nullptr;
     if (opt_.filter_policy != YBGPU_FILTER_NONE) {
       if (opt_.filter_policy != YBGPU_FILTER_DOCKEY_V3) return Fail(YBGPU_INVALID_ARGUMENT, "unknown filter_policy");
-      CUDA_TRY(DevAlloc(&I.allocs, &E.fk_len, n));
+      CUDA_TRY(DevAlloc(&I.mem, &E.fk_len, n));
       E.fk_src = d_fk16;
       E.fkh_src = d_fkh;
     }
-    CUDA_TRY(DevAlloc(&I.allocs, &E.max_add, 1));
+    CUDA_TRY(DevAlloc(&I.mem, &E.max_add, 1));
     CUDA_TRY(cudaMemsetAsync(E.max_add, 0, 4, I.stream));
     // ---- block planning: per-entry sizes with the chunk partials of P, QQ and the filter-key ordinals in one pass, one scan
     // launch over all partial arrays, one launch that applies them (encode_kernels.cuh)
@@ -2435,18 +2527,18 @@ ybgpu_status Engine::Run(const volatile int32_t* shutting_down) {
     unsigned long long *d_pp = nullptr, *d_qp = nullptr;
     uint32_t* d_counts = nullptr;                         // [0] data blocks, [1] distinct filter keys
     uint8_t* d_is_new = nullptr; uint32_t* d_npart = nullptr; uint32_t* d_new_entry = nullptr; uint32_t* d_hash = nullptr;
-    CUDA_TRY(DevAlloc(&I.allocs, &d_pp, pc + 1));
-    CUDA_TRY(DevAlloc(&I.allocs, &d_qp, static_cast<size_t>(qchunks) * ri + 1));
-    CUDA_TRY(DevAlloc(&I.allocs, &d_counts, 2));
+    CUDA_TRY(DevAlloc(&I.mem, &d_pp, pc + 1));
+    CUDA_TRY(DevAlloc(&I.mem, &d_qp, static_cast<size_t>(qchunks) * ri + 1));
+    CUDA_TRY(DevAlloc(&I.mem, &d_counts, 2));
     CUDA_TRY(cudaMemsetAsync(d_counts, 0, 8, I.stream));
     host::FilterGeometry hg{};
     if (E.fk_len) {
       hg = host::ComputeFilterGeometry(opt_.filter_block_size ? opt_.filter_block_size : 65536u);
       if (hg.max_keys == 0) return Fail(YBGPU_INVALID_ARGUMENT, "filter_block_size too small");
-      CUDA_TRY(DevAlloc(&I.allocs, &d_is_new, n)); CUDA_TRY(DevAlloc(&I.allocs, &d_npart, pc + 1));
+      CUDA_TRY(DevAlloc(&I.mem, &d_is_new, n)); CUDA_TRY(DevAlloc(&I.mem, &d_npart, pc + 1));
       // no more distinct filter keys than entries: sized before the count is known, so that one pass can fill both
-      CUDA_TRY(DevAlloc(&I.allocs, &d_new_entry, static_cast<size_t>(n) + 1));
-      if (((hg.filter_bytes + 7u) & ~7u) <= FILTER_SMEM_MAX) CUDA_TRY(DevAlloc(&I.allocs, &d_hash, n));
+      CUDA_TRY(DevAlloc(&I.mem, &d_new_entry, static_cast<size_t>(n) + 1));
+      if (((hg.filter_bytes + 7u) & ~7u) <= FILTER_SMEM_MAX) CUDA_TRY(DevAlloc(&I.mem, &d_hash, n));
     }
     k_plan_entries<<<(n + PLAN_CHUNK - 1) / PLAN_CHUNK, 256, 0, I.stream>>>(E, Sfinal, d_is_new, d_pp, pc, d_qp, qchunks, d_npart);
     k_plan_scan<<<ri + 2, 1024, 0, I.stream>>>(d_pp, pc, d_qp, qchunks, d_npart, d_counts + 1);
@@ -2456,9 +2548,9 @@ ybgpu_status Engine::Run(const volatile int32_t* shutting_down) {
     const uint32_t nsegs = (n + SEG - 1) / SEG;
     const uint32_t ngroups = (nsegs + GROUP_SEGS - 1) / GROUP_SEGS;
     uint32_t *d_gexit = nullptr, *d_group_first = nullptr, *d_seg_first = nullptr, *d_seg_blocks = nullptr;
-    CUDA_TRY(DevAlloc(&I.allocs, &d_gexit, static_cast<size_t>(ngroups) * SEG));
-    CUDA_TRY(DevAlloc(&I.allocs, &d_group_first, ngroups)); CUDA_TRY(DevAlloc(&I.allocs, &d_seg_first, nsegs));
-    CUDA_TRY(DevAlloc(&I.allocs, &d_seg_blocks, nsegs));
+    CUDA_TRY(DevAlloc(&I.mem, &d_gexit, static_cast<size_t>(ngroups) * SEG));
+    CUDA_TRY(DevAlloc(&I.mem, &d_group_first, ngroups)); CUDA_TRY(DevAlloc(&I.mem, &d_seg_first, nsegs));
+    CUDA_TRY(DevAlloc(&I.mem, &d_seg_blocks, nsegs));
     k_seg_exit<<<nsegs, 256, 0, I.stream>>>(E);
     k_group_exit<<<static_cast<uint32_t>((static_cast<uint64_t>(ngroups) * SEG + 255) / 256), 256, 0, I.stream>>>(E, d_gexit, ngroups);
     k_chain_groups<<<1, 32, 0, I.stream>>>(E, d_gexit, ngroups, d_group_first);
@@ -2470,16 +2562,16 @@ ybgpu_status Engine::Run(const volatile int32_t* shutting_down) {
     if (ybgpu_status s = ReadSmall(counts, d_counts, 8)) return s;
     const uint32_t nblocks = counts[0], n_keys = counts[1];
     I.n_blocks = nblocks;
-    CUDA_TRY(DevAlloc(&I.allocs, &I.d_block_first, static_cast<size_t>(nblocks) + 1));
-    CUDA_TRY(DevAlloc(&I.allocs, &I.d_block_off, static_cast<size_t>(nblocks) + 1));
+    CUDA_TRY(DevAlloc(&I.mem, &I.d_block_first, static_cast<size_t>(nblocks) + 1));
+    CUDA_TRY(DevAlloc(&I.mem, &I.d_block_off, static_cast<size_t>(nblocks) + 1));
     unsigned long long* d_total = nullptr;                // [0] file length, [1] largest block (contents + trailer)
-    CUDA_TRY(DevAlloc(&I.allocs, &d_total, 2));
+    CUDA_TRY(DevAlloc(&I.mem, &d_total, 2));
     CUDA_TRY(cudaMemsetAsync(d_total, 0, 16, I.stream));
     k_block_fill<<<(nsegs + 127) / 128, 128, 0, I.stream>>>(E, d_seg_first, nsegs, d_seg_blocks, I.d_block_first, I.d_block_off, d_total + 1);
     {
       const uint32_t bc = (nblocks + SCAN_CHUNK - 1) / SCAN_CHUNK;
       unsigned long long* d_bpart = nullptr;
-      CUDA_TRY(DevAlloc(&I.allocs, &d_bpart, static_cast<size_t>(bc) + 1));
+      CUDA_TRY(DevAlloc(&I.mem, &d_bpart, static_cast<size_t>(bc) + 1));
       k_u64_chunk_sums<<<bc, 256, 0, I.stream>>>(I.d_block_off, nblocks, d_bpart);
       k_scan_u64_single<<<1, 1024, 0, I.stream>>>(d_bpart, bc, d_total);
       k_u64_chunk_final<<<bc, 256, 0, I.stream>>>(I.d_block_off, nblocks, d_bpart);
@@ -2490,7 +2582,7 @@ ybgpu_status Engine::Run(const volatile int32_t* shutting_down) {
     const unsigned long long total = total_and_max[0];
     if (ybgpu_status us = UploadSmall(I.d_block_off + nblocks, &total, 8)) return us;
     I.out_file_len = total;
-    CUDA_TRY(DevAlloc(&I.allocs, &I.out_file, total + 64));
+    CUDA_TRY(DevAlloc(&I.mem, &I.out_file, total + 64));
     {
       const size_t esm = ENC_SMEM_CAP + 32;
       const bool tsp = E.key_encoding == YBGPU_KEY_ENCODING_THREE_SHARED_PARTS;
@@ -2538,11 +2630,11 @@ ybgpu_status Engine::Run(const volatile int32_t* shutting_down) {
       C.raw = I.out_file; C.raw_off = I.d_block_off; C.nblocks = nblocks;
       unsigned long long* d_foff = nullptr; unsigned long long* d_ftotal = nullptr; unsigned long long* d_fpart = nullptr;
       const uint32_t bc = (nblocks + SCAN_CHUNK - 1) / SCAN_CHUNK;
-      CUDA_TRY(DevAlloc(&I.allocs, &C.comp, total + 64));
-      CUDA_TRY(DevAlloc(&I.allocs, &C.csize, nblocks));
-      CUDA_TRY(DevAlloc(&I.allocs, &d_foff, static_cast<size_t>(nblocks) + 1));
-      CUDA_TRY(DevAlloc(&I.allocs, &d_ftotal, 1));
-      CUDA_TRY(DevAlloc(&I.allocs, &d_fpart, static_cast<size_t>(bc) + 1));
+      CUDA_TRY(DevAlloc(&I.mem, &C.comp, total + 64));
+      CUDA_TRY(DevAlloc(&I.mem, &C.csize, nblocks));
+      CUDA_TRY(DevAlloc(&I.mem, &d_foff, static_cast<size_t>(nblocks) + 1));
+      CUDA_TRY(DevAlloc(&I.mem, &d_ftotal, 1));
+      CUDA_TRY(DevAlloc(&I.mem, &d_fpart, static_cast<size_t>(bc) + 1));
       C.fsize = d_foff;
       const uint32_t cgrid = std::min<uint32_t>((nblocks + SNAPC_WARPS - 1) / SNAPC_WARPS, static_cast<uint32_t>(sms) * 4);
       // A/B switch (same binary): how the encoder forms the hash groups of a batch, see snapc_prepare
@@ -2580,7 +2672,7 @@ ybgpu_status Engine::Run(const volatile int32_t* shutting_down) {
       unsigned long long ftotal = 0;
       if (ybgpu_status s = ReadSmall(&ftotal, d_ftotal, 8)) return s;
       if (ybgpu_status us = UploadSmall(d_foff + nblocks, &ftotal, 8)) return us;
-      CUDA_TRY(DevAlloc(&I.allocs, &C.out, ftotal + 64));
+      CUDA_TRY(DevAlloc(&I.mem, &C.out, ftotal + 64));
       CUDA_TRY(cudaEventRecord(I.snap_ev[2], I.stream));
       k_snappy_gather<<<GridFor(static_cast<uint64_t>(nblocks) * 32, 256, sms), 256, 0, I.stream>>>(C);
       CUDA_TRY(cudaEventRecord(I.snap_ev[3], I.stream));
@@ -2589,10 +2681,7 @@ ybgpu_status Engine::Run(const volatile int32_t* shutting_down) {
       stats_.path_flags |= lz4_out ? YBGPU_PATH_LZ4_OUTPUT : YBGPU_PATH_SNAPPY_OUTPUT;
       // the uncompressed table and the scratch image are done with once the gather has run (stream-ordered frees): the job's
       // footprint stays at one output table for the later phases and for the jobs running beside this one
-      for (void* dead : {static_cast<void*>(I.out_file), static_cast<void*>(C.comp)}) {
-        auto it = std::find(I.allocs.begin(), I.allocs.end(), dead);
-        if (it != I.allocs.end()) { I.allocs.erase(it); CUDA_TRY(cudaFreeAsync(dead, I.stream)); }
-      }
+      for (void* dead : {static_cast<void*>(I.out_file), static_cast<void*>(C.comp)}) CUDA_TRY(I.mem.Free(dead, I.stream));
       I.out_file = C.out; I.out_file_len = ftotal; I.d_block_off = d_foff;
     }
     if (E.fk_len) {
@@ -2602,9 +2691,9 @@ ybgpu_status Engine::Run(const volatile int32_t* shutting_down) {
       const uint32_t nfb = std::max<uint32_t>(1, (n_keys + g.max_keys - 1) / g.max_keys);
       I.n_filter_blocks = nfb; I.filter_block_bytes = g.block_bytes;
       I.filter_key_stride = static_cast<uint32_t>((max_ikey + 2 + 7) & ~7u);
-      CUDA_TRY(DevAlloc(&I.allocs, &I.d_filters, static_cast<size_t>(nfb) * g.dev_stride + 16));
-      CUDA_TRY(DevAlloc(&I.allocs, &I.d_filter_keys, static_cast<size_t>(nfb) * 2 * I.filter_key_stride));
-      CUDA_TRY(DevAlloc(&I.allocs, &I.d_filter_first, nfb));
+      CUDA_TRY(DevAlloc(&I.mem, &I.d_filters, static_cast<size_t>(nfb) * g.dev_stride + 16));
+      CUDA_TRY(DevAlloc(&I.mem, &I.d_filter_keys, static_cast<size_t>(nfb) * 2 * I.filter_key_stride));
+      CUDA_TRY(DevAlloc(&I.mem, &I.d_filter_first, nfb));
       CUDA_TRY(cudaMemsetAsync(I.d_filters, 0, static_cast<size_t>(nfb) * g.dev_stride, I.stream));
       if (n_keys && d_hash) {
         CUDA_TRY(cudaFuncSetAttribute(k_filter_build_smem, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(g.dev_stride)));
@@ -2621,8 +2710,8 @@ ybgpu_status Engine::Run(const volatile int32_t* shutting_down) {
     if (opt_.compute_user_boundary_values && opt_.retention_enabled) {
       const int bgrid = static_cast<int>(std::max<uint64_t>(1, std::min<uint64_t>((n + 255) / 256, static_cast<uint64_t>(sms) * 2)));
       BvCand* d_cand = nullptr;
-      CUDA_TRY(DevAlloc(&I.allocs, &d_cand, static_cast<size_t>(bgrid) * 2 * BV_MAXC));
-      CUDA_TRY(DevAlloc(&I.allocs, &I.d_bv, 1));
+      CUDA_TRY(DevAlloc(&I.mem, &d_cand, static_cast<size_t>(bgrid) * 2 * BV_MAXC));
+      CUDA_TRY(DevAlloc(&I.mem, &I.d_bv, 1));
       CUDA_TRY(cudaMemsetAsync(d_cand, 0, sizeof(BvCand) * static_cast<size_t>(bgrid) * 2 * BV_MAXC, I.stream));
       CUDA_TRY(cudaMemsetAsync(I.d_bv, 0, sizeof(BvOut), I.stream));
       k_boundary_values<<<bgrid, 256, 0, I.stream>>>(E, Sfinal, d_cand, I.d_bv);
@@ -2631,7 +2720,7 @@ ybgpu_status Engine::Run(const volatile int32_t* shutting_down) {
     }
     I.boundary_stride = static_cast<uint32_t>((max_ikey + 2 + 7) & ~7u);
     // slot 2*nblocks (one past the per-block pairs): the first key of the file (FileMetaData::smallest)
-    CUDA_TRY(DevAlloc(&I.allocs, &I.d_boundary, (static_cast<size_t>(nblocks) * 2 + 1) * I.boundary_stride));
+    CUDA_TRY(DevAlloc(&I.mem, &I.d_boundary, (static_cast<size_t>(nblocks) * 2 + 1) * I.boundary_stride));
     k_boundary_keys<<<GridFor(static_cast<uint64_t>(nblocks) * 2 + 1, 256, sms), 256, 0, I.stream>>>(E, Sfinal, I.d_block_first, nblocks, I.d_boundary, I.boundary_stride);
     launches++;
   }
@@ -2704,10 +2793,10 @@ ybgpu_status Engine::EnsureKvStream() {
   if (I.kv_emitted) return YBGPU_OK;
   CUDA_TRY(cudaSetDevice(opt_.device));
   g_alloc_stream = I.stream;
-  CUDA_TRY(DevAlloc(&I.allocs, &I.out_keys, I.out_key_bytes + 16));
-  CUDA_TRY(DevAlloc(&I.allocs, &I.out_vals, I.out_val_bytes + 16));
-  CUDA_TRY(DevAlloc(&I.allocs, &I.out_koff, I.n_out + 1));
-  CUDA_TRY(DevAlloc(&I.allocs, &I.out_voff, I.n_out + 1));
+  CUDA_TRY(DevAlloc(&I.mem, &I.out_keys, I.out_key_bytes + 16));
+  CUDA_TRY(DevAlloc(&I.mem, &I.out_vals, I.out_val_bytes + 16));
+  CUDA_TRY(DevAlloc(&I.mem, &I.out_koff, I.n_out + 1));
+  CUDA_TRY(DevAlloc(&I.mem, &I.out_voff, I.n_out + 1));
   if (I.N) {
     if (!I.partial_ready) { if (ybgpu_status s = EnsureChunkSums()) return s; stats_.gpu_kernel_launches += 2; }
     EmitView ev{};
@@ -2870,14 +2959,15 @@ ybgpu_status Engine::Digest(uint64_t* digest) {
 namespace {
 // Temporaries of one check, from the stream-ordered pool; returned to it when the check ends, however it ends.
 struct VerifyScratch {
+  JobMemory& mem;
   cudaStream_t stream;
   std::vector<void*> ptrs;
-  explicit VerifyScratch(cudaStream_t s) : stream(s) {}
-  ~VerifyScratch() { for (void* p : ptrs) cudaFreeAsync(p, stream); }
+  VerifyScratch(JobMemory& m, cudaStream_t s) : mem(m), stream(s) {}
+  ~VerifyScratch() { for (void* p : ptrs) mem.Free(p, stream); }
   template <typename T>
   cudaError_t Alloc(T** out, size_t count) {
     void* p = nullptr;
-    cudaError_t e = cudaMallocAsync(&p, std::max<size_t>(count * sizeof(T), 16) + 32, stream);
+    cudaError_t e = mem.Alloc(&p, JobMemory::Padded(count * sizeof(T)), stream);
     if (e == cudaSuccess) { ptrs.push_back(p); *out = reinterpret_cast<T*>(p); }
     return e;
   }
@@ -2905,7 +2995,7 @@ ybgpu_status Engine::VerifyTable(const uint8_t* file, uint64_t file_len, const u
   if (nb == 0) return YBGPU_OK;                            // no table was written (compaction_job.cc:950-952)
   int sms = 0;
   CUDA_TRY(EnsureDeviceTables(opt_.device, I.stream, &sms));
-  VerifyScratch T(I.stream);
+  VerifyScratch T(I.mem, I.stream);
   cudaEvent_t ev[2] = {};
   for (auto& e : ev) CUDA_TRY(cudaEventCreate(&e));
   struct EvGuard { cudaEvent_t* e; ~EvGuard() { cudaEventDestroy(e[0]); cudaEventDestroy(e[1]); } } ev_guard{ev};
@@ -3025,7 +3115,7 @@ ybgpu_status Engine::VerifySst(const uint8_t* data, uint64_t len, const ybgpu_bl
   }
   if (nh == 0) return YBGPU_OK;
   CUDA_TRY(cudaSetDevice(opt_.device));
-  VerifyScratch T(I.stream);
+  VerifyScratch T(I.mem, I.stream);
   uint8_t* d = nullptr; unsigned long long* d_off = nullptr; uint32_t* d_sz = nullptr;
   CUDA_TRY(T.Alloc(&d, len + 64)); CUDA_TRY(T.Alloc(&d_off, nh)); CUDA_TRY(T.Alloc(&d_sz, nh));
   CUDA_TRY(cudaMemsetAsync(d, 0, 16, I.stream));

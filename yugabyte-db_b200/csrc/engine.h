@@ -1,5 +1,6 @@
 // engine.h — host-side interface of the CUDA engine (implementation: engine.cu).
 #pragma once
+#include <mutex>
 #include <string>
 #include <vector>
 
@@ -9,6 +10,22 @@
 namespace ybgpu {
 
 constexpr int MAX_RUNS = 64;   // input files per job (configs use 2..32)
+// opens the message of every failure caused by ybgpu_job_options::device_memory_budget (before upload or during run)
+constexpr char kBudgetExceeded[] = "device memory budget exceeded";
+
+// Device bytes held at once by a set of jobs (the ranges of one pipelined compaction): every allocation and free of a
+// member job updates `in_use` when it happens, so `peak` is the high-water mark of the jobs' bytes live together.
+struct MemGroup {
+  std::mutex mu;
+  uint64_t in_use = 0, peak = 0;
+  void Change(int64_t delta) {
+    std::lock_guard<std::mutex> l(mu);
+    in_use += delta;
+    if (in_use > peak) peak = in_use;
+  }
+};
+// Makes `job` (a ybgpu_job of this library) a member of `group` from now until it is destroyed; its bytes held so far count.
+void JoinMemGroup(ybgpu_job* job, MemGroup* group);
 
 class Engine {
  public:
@@ -18,6 +35,7 @@ class Engine {
   ybgpu_status AddInput(const uint8_t* data, uint64_t len, const ybgpu_block_handle* handles, uint64_t nh,
                         int key_encoding, uint64_t ht_filter, bool on_device);
   ybgpu_status AddInputKv(const uint8_t* keys, const uint64_t* key_offsets, const uint8_t* values, const uint64_t* value_offsets, uint64_t n);
+  void JoinMemGroup(MemGroup* group);
   ybgpu_status SetCotableFilters(const uint32_t* db_oids, const uint64_t* hybrid_times, uint32_t n);
   ybgpu_status WaitInputs();
   ybgpu_status Run(const volatile int32_t* shutting_down);
@@ -47,15 +65,18 @@ class Engine {
   ybgpu_status VerifySst(const uint8_t* data, uint64_t len, const ybgpu_block_handle* handles, uint64_t nh, int key_encoding,
                          ybgpu_output_check* result);
   const ybgpu_job_options& options() const { return opt_; }
-  ybgpu_job_stats& stats() { return stats_; }
+  ybgpu_job_stats& stats();
   const std::string& error() const { return error_; }
   ybgpu_status Fail(ybgpu_status s, const std::string& msg);
+  // a failed CUDA call (cudaError_t e); a request the job's device_memory_budget refused gets the budget message
+  ybgpu_status FailCuda(const char* expr, int e);
   bool ran() const { return ran_; }
   int record_stride() const { return record_stride_; }
   uint32_t num_tiles() const { return num_tiles_; }
 
  private:
   ybgpu_status CheckDeviceError(const char* phase);
+  ybgpu_status CheckBudgetBeforeUpload(uint64_t more);
   ybgpu_status ReadSmall(void* host_dst, const void* dev_src, size_t n);
   ybgpu_status UploadSmall(void* dev_dst, const void* host_src, size_t n);
   ybgpu_status ReadViaMapped(void* host_dst, const void* dev_src, size_t row_bytes, size_t src_pitch, size_t rows);

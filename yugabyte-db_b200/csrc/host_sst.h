@@ -24,6 +24,31 @@ struct Handle { uint64_t offset = 0, size = 0; };
 // rocksdb::CompressionType — 1 Snappy, 4 LZ4, 5 LZ4HC (the same stream format). False on a malformed stream or another
 // codec.
 bool UncompressStoredBlock(uint8_t type, const uint8_t* stored, size_t n, std::string* out);
+// The uncompressed image the engine builds when any input block is stored compressed (k_snappy_sizes): every block's
+// contents + its 5-byte trailer, the contents' size read from the varint32 preamble of a Snappy / LZ4 / LZ4HC block (the
+// stored size for a raw one), the way ybgpu_sst_check_supported reads trailers. `compressed` receives the number of
+// blocks stored compressed. Handles (Handle or ybgpu_block_handle) must lie inside the file (checked by the callers).
+template <typename H>
+uint64_t UncompressedImageBytes(const uint8_t* data, const H* blocks, uint64_t n, uint64_t* compressed) {
+  uint64_t total = 0, nc = 0;
+  for (uint64_t i = 0; i < n; i++) {
+    const uint8_t* p = data + blocks[i].offset;
+    const uint64_t size = blocks[i].size;
+    const uint8_t type = p[size];
+    uint64_t u = size;
+    if (type == 1 || type == 4 || type == 5) {          // Snappy, LZ4, LZ4HC: varint32 preamble
+      nc++;
+      u = 0;
+      for (uint64_t j = 0; j < 5 && j < size; j++) {
+        u |= static_cast<uint64_t>(p[j] & 127) << (7 * j);
+        if (!(p[j] & 128)) break;
+      }
+    }
+    total += u + 5;
+  }
+  *compressed = nc;
+  return total;
+}
 uint32_t Crc32c(const uint8_t* p, size_t n, uint32_t init = 0);   // rocksdb/util/crc32c.h Extend
 inline uint32_t Crc32cMask(uint32_t c) { return ((c >> 15) | (c << 17)) + 0xa282ead8u; }
 

@@ -16,6 +16,7 @@
 #include <cstdlib>
 #include <cstdio>
 #include <cstring>
+#include <functional>
 #include <mutex>
 #include <string>
 #include <thread>
@@ -24,6 +25,7 @@
 #include "../../include/ybgpu_compaction.h"
 #include "dev_logic.cuh"
 #include "host_sst.h"
+#include "engine.h"
 #include "range_plan.h"
 
 namespace ybgpu {
@@ -85,6 +87,23 @@ void CollectSamples(const std::vector<ParsedInput>& in, uint32_t n_ranges, std::
   }
 }
 
+bool RowPrefix(const std::string& k, bool docdb_keys, std::string* cut) {
+  int plen = static_cast<int>(k.size());
+  if (docdb_keys) {
+    // group_prefix_len scans with aligned 8-byte loads: give it an aligned, padded copy
+    alignas(8) uint8_t buf[1040];
+    if (k.size() > 1024) return false;
+    memset(buf, 0, sizeof(buf));
+    memcpy(buf, k.data(), k.size());
+    plen = ybgpu::group_prefix_len(buf, static_cast<int>(k.size()), true);
+    if (plen == -ybgpu::DEV_ERR_UNSUPPORTED_KEY) return false;
+    if (plen <= 0) plen = static_cast<int>(k.size());
+  }
+  if (plen == 0 || plen > YBGPU_MAX_SPLITTER_LEN) return false;
+  *cut = k.substr(0, plen);
+  return true;
+}
+
 std::vector<std::string> SplittersFromSamples(std::vector<Sample> samples, uint32_t n_ranges, bool docdb_keys) {
   std::vector<std::string> out;
   if (n_ranges <= 1 || samples.empty()) return out;
@@ -96,25 +115,35 @@ std::vector<std::string> SplittersFromSamples(std::vector<Sample> samples, uint3
   for (const Sample& s : samples) {
     acc += static_cast<double>(s.w);
     if (acc < next || out.size() + 1 >= n_ranges) continue;
-    const std::string& k = s.key;
-    int plen = static_cast<int>(k.size());
-    if (docdb_keys) {
-      // group_prefix_len scans with aligned 8-byte loads: give it an aligned, padded copy
-      alignas(8) uint8_t buf[1040];
-      if (k.size() > 1024) continue;
-      memset(buf, 0, sizeof(buf));
-      memcpy(buf, k.data(), k.size());
-      plen = ybgpu::group_prefix_len(buf, static_cast<int>(k.size()), true);
-      if (plen == -ybgpu::DEV_ERR_UNSUPPORTED_KEY) continue;
-      if (plen <= 0) plen = static_cast<int>(k.size());
-    }
-    if (plen == 0 || plen > YBGPU_MAX_SPLITTER_LEN) continue;
-    std::string cut = k.substr(0, plen);
+    std::string cut;
+    if (!RowPrefix(s.key, docdb_keys, &cut)) continue;
     if (!out.empty() && !(out.back() < cut)) continue;
     out.push_back(cut);
     next = target * static_cast<double>(out.size() + 1);
   }
   return out;
+}
+
+// The samples of the blocks that can hold keys of [lo, hi), already cut to their row prefix and kept only when that
+// prefix lies strictly inside the range, then the weighted median of them.
+bool SplitRange(const std::vector<ParsedInput>& in, const std::string& lo, const std::string& hi, bool docdb_keys, std::string* mid) {
+  std::vector<Sample> samples;
+  for (const ParsedInput& p : in) {
+    size_t a, b;
+    BlocksForRange(p.useps, lo, hi, &a, &b);
+    uint64_t w = 0;
+    for (size_t i = a; i < b; i++) {
+      w += p.meta.data_blocks[i].size + 5;
+      std::string cut;
+      if (!RowPrefix(p.useps[i], docdb_keys, &cut) || !(lo < cut) || (!hi.empty() && !(cut < hi))) continue;
+      samples.push_back({cut, w});
+      w = 0;
+    }
+  }
+  const std::vector<std::string> sp = SplittersFromSamples(std::move(samples), 2, false);
+  if (sp.empty()) return false;
+  *mid = sp[0];
+  return true;
 }
 
 std::vector<std::string> PlanSplitters(const std::vector<ParsedInput>& in, uint32_t n_ranges, bool docdb_keys) {
@@ -297,6 +326,20 @@ ybgpu_status ybgpu_plan_subcompactions(const ybgpu_input_file* files, uint32_t n
   return YBGPU_OK;
 }
 
+ybgpu_status ybgpu_split_range(const ybgpu_input_file* files, uint32_t num_files, int32_t docdb_keys, const uint8_t* lower,
+                               uint32_t lower_len, const uint8_t* upper, uint32_t upper_len, uint8_t* splitter, uint32_t* splitter_len) {
+  if (!files || !splitter || !splitter_len || (lower_len && !lower) || (upper_len && !upper)) return YBGPU_INVALID_ARGUMENT;
+  std::vector<ParsedInput> in;
+  std::string err;
+  if (!ParseInputs(files, num_files, &in, &err)) return YBGPU_CORRUPTION;
+  std::string mid;
+  const std::string lo(reinterpret_cast<const char*>(lower), lower_len), hi(reinterpret_cast<const char*>(upper), upper_len);
+  if (!SplitRange(in, lo, hi, docdb_keys != 0, &mid)) return YBGPU_NOT_FOUND;
+  memcpy(splitter, mid.data(), mid.size());
+  *splitter_len = static_cast<uint32_t>(mid.size());
+  return YBGPU_OK;
+}
+
 }  // extern "C"
 
 namespace {
@@ -323,11 +366,27 @@ ybgpu_status CompactFilesCore(const ybgpu_job_options* options, const ybgpu_inpu
   if (options->range_lower_len || options->range_upper_len) return fail(YBGPU_INVALID_ARGUMENT, "range bounds are set by the subcompaction planner");
   if (!ybgpu::host::OutputCompressionSupported(options->output_compression))
     return fail(YBGPU_NOT_SUPPORTED, ybgpu::host::UnsupportedOutputCompression(options->output_compression));
-  if (max_subcompactions == 0) max_subcompactions = 1;
+  const uint64_t budget = options->device_memory_budget;
+  if (max_subcompactions == 0 && !budget) max_subcompactions = 1;
+  const uint32_t output_slots = budget && !one ? *num_outputs : max_subcompactions;
   if (max_in_flight == 0) max_in_flight = 3;
+  // every range runs as a job with this budget (its reservation until it has run)
+  const uint64_t job_budget = budget ? std::max<uint64_t>(1, budget / max_in_flight) : 0;
   std::vector<ParsedInput> in;
   std::string perr;
   if (!ParseInputs(files, num_files, &in, &perr)) return fail(YBGPU_CORRUPTION, perr);
+  if (max_subcompactions == 0) {
+    // as many ranges as the budget needs: about a third of a range's budget in input bytes (inputs + uncompressed image);
+    // a range that needs more is cut again when it runs
+    uint64_t known = 0;
+    for (uint32_t f = 0; f < num_files; f++) {
+      uint64_t comp = 0;
+      const uint64_t img = ybgpu::host::UncompressedImageBytes(files[f].data_file, in[f].meta.data_blocks.data(), in[f].meta.data_blocks.size(), &comp);
+      known += files[f].data_file_len + (comp ? img : 0);
+    }
+    const uint64_t per_range = std::max<uint64_t>(1, job_budget / 3);
+    max_subcompactions = static_cast<uint32_t>(std::min<uint64_t>(1u << 16, std::max<uint64_t>(1, (known + per_range - 1) / per_range)));
+  }
 
   // Compaction::GetLargestUserKey (db/compaction.cc:318): the seqno-zeroing exception key is a
   // property of the whole compaction, not of a range.
@@ -345,15 +404,31 @@ ybgpu_status CompactFilesCore(const ybgpu_job_options* options, const ybgpu_inpu
     }
   }
 
-  const std::vector<std::string> splitters = PlanSplitters(in, max_subcompactions, options->retention_enabled != 0);
+  const bool docdb_keys = options->retention_enabled != 0;
+  const std::vector<std::string> splitters = PlanSplitters(in, max_subcompactions, docdb_keys);
   const uint32_t n_ranges = static_cast<uint32_t>(splitters.size()) + 1;
+  if (n_ranges > output_slots && !one) return fail(YBGPU_INVALID_ARGUMENT, "more ranges than output slots");
   *num_outputs = n_ranges;
-  for (uint32_t r = 0; r < n_ranges; r++) {
-    ybgpu_sub_output& o = outputs[r];
-    memset(&o, 0, sizeof(o));
-    if (r > 0) { o.range_lower_len = static_cast<uint32_t>(splitters[r - 1].size()); memcpy(o.range_lower, splitters[r - 1].data(), splitters[r - 1].size()); }
-    if (r + 1 < n_ranges) { o.range_upper_len = static_cast<uint32_t>(splitters[r].size()); memcpy(o.range_upper, splitters[r].data(), splitters[r].size()); }
-  }
+  // the outputs of every planned range in key order: one, or more when the range was cut to fit the budget
+  std::vector<std::vector<ybgpu_sub_output>> subs(n_ranges);
+
+  // device_memory_budget: ranges are admitted in range order while the reservations on the device leave room; a range
+  // holds job_budget until it has run, then its measured peak until its job is destroyed
+  std::mutex res_mu;
+  std::condition_variable res_cv;
+  uint64_t reserved = 0;
+  auto reserve = [&](uint64_t x) {
+    std::unique_lock<std::mutex> l(res_mu);
+    res_cv.wait(l, [&] { return reserved + x <= budget; });
+    reserved += x;
+  };
+  auto unreserve = [&](uint64_t x) {
+    { std::lock_guard<std::mutex> l(res_mu); reserved -= x; }
+    res_cv.notify_all();
+  };
+  // every range job counts its allocations and frees here as well: total.device_bytes_peak is the high-water mark of the
+  // bytes the ranges hold at once
+  ybgpu::MemGroup mem_group;
 
   std::atomic<uint32_t> next_range{0};
   std::atomic<uint64_t> data_used{0}, meta_used{0};
@@ -365,9 +440,10 @@ ybgpu_status CompactFilesCore(const ybgpu_job_options* options, const ybgpu_inpu
   std::mutex ot_mu;
   std::condition_variable ot_cv;
   std::vector<int> ot_state(one ? n_ranges : 0, 0);
-  std::vector<uint64_t> ot_dlen(one ? n_ranges : 0, 0);
-  std::vector<std::string> ot_meta(one ? n_ranges : 0);
+  std::vector<uint64_t> ot_dlen(one ? n_ranges : 0, 0);             // the range's data bytes, all its pieces
+  std::vector<std::vector<std::string>> ot_meta(one ? n_ranges : 0); // per piece of the range
   uint32_t ot_next = 0;
+  size_t ot_next_piece = 0;
   std::unique_ptr<ybgpu::host::ConcatBuilder> ot_builder;
   std::string ot_error;
   auto record_failure = [&](ybgpu_status s, const std::string& msg) {
@@ -388,12 +464,25 @@ ybgpu_status CompactFilesCore(const ybgpu_job_options* options, const ybgpu_inpu
     for (uint32_t f = 0; f < num_files; f++) in_meta += files[f].meta_file_len;
     ot_builder->Reserve(in_meta + in_meta / 4 + 65536);
   }
-  auto ot_piece = [&](uint32_t r) {
+  auto ot_piece = [&](uint32_t r, size_t i) {
+    const ybgpu_sub_output& o = subs[r][i];
     ybgpu::host::SstPiece p;
-    p.meta = reinterpret_cast<const uint8_t*>(ot_meta[r].data()); p.meta_len = ot_meta[r].size(); p.data_len = ot_dlen[r];
-    p.smallest.assign(reinterpret_cast<const char*>(outputs[r].smallest_key), outputs[r].smallest_key_len);
-    p.largest.assign(reinterpret_cast<const char*>(outputs[r].largest_key), outputs[r].largest_key_len);
+    p.meta = reinterpret_cast<const uint8_t*>(ot_meta[r][i].data()); p.meta_len = ot_meta[r][i].size(); p.data_len = o.data_len;
+    p.smallest.assign(reinterpret_cast<const char*>(o.smallest_key), o.smallest_key_len);
+    p.largest.assign(reinterpret_cast<const char*>(o.largest_key), o.largest_key_len);
     return p;
+  };
+  // With ot_mu held: the first piece with data at or after piece i of range a -> (*ra, *ri); false when a range on the way
+  // has not completed. (*ra == n_ranges: none is left.)
+  auto ot_seek = [&](uint32_t a, size_t i, uint32_t* ra, size_t* ri) {
+    for (; a < n_ranges; a++, i = 0) {
+      *ra = a; *ri = i;
+      if (ot_state[a] != 2) return false;
+      for (; i < subs[a].size(); i++)
+        if (subs[a][i].data_len) { *ri = i; return true; }
+    }
+    *ra = n_ranges; *ri = 0;
+    return true;
   };
   // Called with ot_mu held (through `lock`): feeds every piece whose successor is known to the builder, in key order.
   // The assembly itself (index keys rebased, separators recomputed: milliseconds per piece) runs WITHOUT ot_mu — the
@@ -404,16 +493,14 @@ ybgpu_status CompactFilesCore(const ybgpu_job_options* options, const ybgpu_inpu
     if (ot_building) return;
     ot_building = true;
     while (ot_error.empty()) {
-      uint32_t a = ot_next;
-      while (a < n_ranges && ot_state[a] == 2 && ot_dlen[a] == 0) a++;
+      uint32_t a, nx;
+      size_t i, ni;
+      if (!ot_seek(ot_next, ot_next_piece, &a, &i)) break;
       if (a >= n_ranges) { ot_next = n_ranges; break; }
-      if (ot_state[a] != 2) break;
-      uint32_t nx = a + 1;
-      while (nx < n_ranges && ot_state[nx] == 2 && ot_dlen[nx] == 0) nx++;
-      if (nx < n_ranges && ot_state[nx] != 2) break;               // the successor's first key is not known yet
-      const ybgpu::host::SstPiece pa = ot_piece(a);
+      if (!ot_seek(a, i + 1, &nx, &ni)) break;                      // the successor's first key is not known yet
+      const ybgpu::host::SstPiece pa = ot_piece(a, i);
       ybgpu::host::SstPiece pn;
-      if (nx < n_ranges) pn = ot_piece(nx);
+      if (nx < n_ranges) pn = ot_piece(nx, ni);
       lock.unlock();
       std::string e = ot_builder->AddPiece(pa, nx < n_ranges ? &pn : nullptr);
       lock.lock();
@@ -421,8 +508,8 @@ ybgpu_status CompactFilesCore(const ybgpu_job_options* options, const ybgpu_inpu
       if (one->pieces == 0) one->smallest = pa.smallest;
       one->largest = pa.largest;
       one->pieces++;
-      std::string().swap(ot_meta[a]);                               // the piece's own metadata file is no longer needed
-      ot_next = nx;
+      std::string().swap(ot_meta[a][i]);                            // the piece's own metadata file is no longer needed
+      ot_next = nx; ot_next_piece = ni;
     }
     ot_building = false;
   };
@@ -463,135 +550,192 @@ ybgpu_status CompactFilesCore(const ybgpu_job_options* options, const ybgpu_inpu
   std::mutex order_mu; std::condition_variable order_cv; uint32_t h2d_next = 0;
 
   auto run_range = [&](uint32_t r) {
-    ybgpu_sub_output& out = outputs[r];
-    // input slot, in range order; every range that was handed out passes here, so nobody waits for a range that gave up
+    // input slot (and, under a budget, the range's reservation), in range order; every range that was handed out passes
+    // here, so nobody waits for a range that gave up
     SlotGuard in_slot, out_slot;
     {
       std::unique_lock<std::mutex> lock(order_mu);
       order_cv.wait(lock, [&] { return h2d_next == r; });
     }
+    uint64_t held = 0;                                        // this range's reservation
+    if (budget) { reserve(job_budget); held = job_budget; }
     in_slot.Take(&h2d_gate);
     {
       std::lock_guard<std::mutex> lock(order_mu);
       h2d_next = r + 1;
     }
     order_cv.notify_all();
-    double t_begin = ms_now(), t_added = 0, t_ran = 0, t_sized = 0, t_d2h = 0, t_fetched = 0;
-    const std::string lo(reinterpret_cast<const char*>(out.range_lower), out.range_lower_len);
-    const std::string hi(reinterpret_cast<const char*>(out.range_upper), out.range_upper_len);
-    ybgpu_job_options o = *options;
-    o.cuda_stream = YBGPU_STREAM_PRIVATE;
-    o.range_lower = out.range_lower; o.range_lower_len = out.range_lower_len;
-    o.range_upper = out.range_upper; o.range_upper_len = out.range_upper_len;
-    o.has_largest_user_key = have_largest ? 1 : 0;
-    o.largest_user_key = reinterpret_cast<const uint8_t*>(largest_user.data());
-    o.largest_user_key_len = largest_user.size();
-    ybgpu_job* job = nullptr;
-    ybgpu_status s = ybgpu_job_create(&o, &job);
-    if (s != YBGPU_OK) { record_failure(s, std::string("create: ") + ybgpu_last_error()); return; }
-    auto job_fail = [&](ybgpu_status st, const char* what) {
-      record_failure(st, std::string(what) + " (range " + std::to_string(r) + "): " + ybgpu_job_error(job));
-      ybgpu_job_destroy(job);
-    };
-    uint32_t added = 0;
-    std::vector<ybgpu_block_handle> h;
+    struct Unreserve { std::function<void()> f; ~Unreserve() { f(); } } unreserve_at_exit{[&] { if (held) unreserve(held); }};
+    // the key ranges still to run for this planned range, the next one at the back: one, unless a job needs more than
+    // its budget and the range is cut in two
+    std::vector<std::pair<std::string, std::string>> todo;
+    todo.emplace_back(r > 0 ? splitters[r - 1] : std::string(), r + 1 < n_ranges ? splitters[r] : std::string());
+    uint64_t r_data = 0;                                      // one-table mode: data bytes of this range's earlier pieces
+    bool first_piece = true;
+    while (!todo.empty()) {
+      const std::string lo = todo.back().first, hi = todo.back().second;
+      todo.pop_back();
+      if (!first_piece) in_slot.Take(&h2d_gate);
+      first_piece = false;
+      ybgpu_sub_output out;
+      memset(&out, 0, sizeof(out));
+      out.range_lower_len = static_cast<uint32_t>(lo.size()); memcpy(out.range_lower, lo.data(), lo.size());
+      out.range_upper_len = static_cast<uint32_t>(hi.size()); memcpy(out.range_upper, hi.data(), hi.size());
+      double t_begin = ms_now(), t_added = 0, t_ran = 0, t_sized = 0, t_d2h = 0, t_fetched = 0;
+      ybgpu_job_options o = *options;
+      o.cuda_stream = YBGPU_STREAM_PRIVATE;
+      o.range_lower = out.range_lower; o.range_lower_len = out.range_lower_len;
+      o.range_upper = out.range_upper; o.range_upper_len = out.range_upper_len;
+      o.has_largest_user_key = have_largest ? 1 : 0;
+      o.largest_user_key = reinterpret_cast<const uint8_t*>(largest_user.data());
+      o.largest_user_key_len = largest_user.size();
+      o.device_memory_budget = job_budget;
+      ybgpu_job* job = nullptr;
+      ybgpu_status s = ybgpu_job_create(&o, &job);
+      if (s != YBGPU_OK) { record_failure(s, std::string("create: ") + ybgpu_last_error()); return; }
+      ybgpu::JoinMemGroup(job, &mem_group);
+      auto destroy = [&]() { ybgpu_job_destroy(job); };
+      // true: the range was cut in two and both halves wait in `todo` (the job needed more than its budget)
+      bool cut = false;
+      // may_cut: the calls that allocate device memory (add_input, run, verify_output); a budget failure anywhere else
+      // fails the compaction like any other error
+      auto job_fail = [&](ybgpu_status st, const char* what, bool may_cut = false) {
+        const std::string msg = ybgpu_job_error(job);
+        destroy();
+        if (may_cut && budget && msg.find(ybgpu::kBudgetExceeded) != std::string::npos) {
+          std::string mid;
+          if (SplitRange(in, lo, hi, docdb_keys, &mid)) {
+            todo.emplace_back(mid, hi);
+            todo.emplace_back(lo, mid);
+            cut = true;
+            return;
+          }
+          record_failure(st, std::string(what) + " (range " + std::to_string(r) + ", no row boundary left to cut it at): " + msg);
+          return;
+        }
+        record_failure(st, std::string(what) + " (range " + std::to_string(r) + "): " + msg);
+      };
+      auto failed_or_cut = [&]() { in_slot.Drop(); return !cut; };
+      uint32_t added = 0;
+      std::vector<ybgpu_block_handle> h;
 
-    // the blocks of every input that can hold keys of the range, plus — for a range that starts inside a cotable —
-    // the blocks with that table's tombstones (SpansForRange); the last span of an input is its range span
-    std::vector<Span> spans;
-    for (uint32_t f = 0; f < num_files; f++) {
-      SpansForRange(in[f], lo, hi, options->retention_enabled != 0, &spans);
-      const auto& blocks = in[f].meta.data_blocks;
-      for (const Span& sp : spans) {
-        const uint64_t start = blocks[sp.a].offset;
-        const uint64_t end = blocks[sp.b - 1].offset + blocks[sp.b - 1].size + 5;
-        h.resize(sp.b - sp.a);
-        for (size_t i = sp.a; i < sp.b; i++) { h[i - sp.a].offset = blocks[i].offset - start; h[i - sp.a].size = blocks[i].size; }
-        s = ybgpu_job_add_input(job, files[f].data_file + start, end - start, h.data(), h.size(), in[f].meta.key_encoding, files[f].hybrid_time_filter);
-        if (s != YBGPU_OK) { job_fail(s, "add_input"); return; }
-        if (files[f].num_cotable_filters) {
-          s = ybgpu_job_set_cotable_filters(job, files[f].cotable_db_oids, files[f].cotable_hybrid_times, static_cast<uint32_t>(files[f].num_cotable_filters));
-          if (s != YBGPU_OK) { job_fail(s, "set_cotable_filters"); return; }
+      // the blocks of every input that can hold keys of the range, plus — for a range that starts inside a cotable —
+      // the blocks with that table's tombstones (SpansForRange); the last span of an input is its range span
+      std::vector<Span> spans;
+      for (uint32_t f = 0; f < num_files; f++) {
+        SpansForRange(in[f], lo, hi, options->retention_enabled != 0, &spans);
+        const auto& blocks = in[f].meta.data_blocks;
+        for (const Span& sp : spans) {
+          const uint64_t start = blocks[sp.a].offset;
+          const uint64_t end = blocks[sp.b - 1].offset + blocks[sp.b - 1].size + 5;
+          h.resize(sp.b - sp.a);
+          for (size_t i = sp.a; i < sp.b; i++) { h[i - sp.a].offset = blocks[i].offset - start; h[i - sp.a].size = blocks[i].size; }
+          s = ybgpu_job_add_input(job, files[f].data_file + start, end - start, h.data(), h.size(), in[f].meta.key_encoding, files[f].hybrid_time_filter);
+          if (s != YBGPU_OK) { job_fail(s, "add_input", true); if (failed_or_cut()) return; break; }
+          if (files[f].num_cotable_filters) {
+            s = ybgpu_job_set_cotable_filters(job, files[f].cotable_db_oids, files[f].cotable_hybrid_times, static_cast<uint32_t>(files[f].num_cotable_filters));
+            if (s != YBGPU_OK) { job_fail(s, "set_cotable_filters"); return; }
+          }
+          added++;
         }
-        added++;
+        if (cut) break;
       }
-    }
-    if (added && h2d_slots) {
-      s = ybgpu_job_wait_inputs(job);
-      if (s != YBGPU_OK) { job_fail(s, "wait_inputs"); return; }
-    }
-    in_slot.Drop();
-    t_added = ms_now();
-    if (added) {
-      s = ybgpu_job_run(job, shutting_down);
-      if (s != YBGPU_OK) { job_fail(s, "run"); return; }
-      if (verify_outputs) {
-        // paranoid_file_checks: the range's table is re-read on its own stream while it is still in device memory; a bad
-        // range fails the compaction before a byte of it reaches the caller's arena
-        ybgpu_output_check chk;
-        s = ybgpu_job_verify_output(job, &chk);
-        if (s != YBGPU_OK) { job_fail(s, "verify_output"); return; }
+      if (cut) continue;
+      if (added && h2d_slots) {
+        s = ybgpu_job_wait_inputs(job);
+        if (s != YBGPU_OK) { job_fail(s, "wait_inputs"); return; }
       }
-      t_ran = ms_now();
-      uint64_t dl = 0, ml = 0;
-      s = ybgpu_job_output_sizes(job, &dl, &ml);
-      if (s != YBGPU_OK) { job_fail(s, "output_sizes"); return; }
-      t_sized = ms_now();
-      uint64_t doff = 0, moff = 0;
-      uint8_t* meta_dst = nullptr;
-      if (one) {
-        // this range's bytes follow those of every earlier range: wait until they all know their sizes
-        std::unique_lock<std::mutex> lock(ot_mu);
-        ot_dlen[r] = dl; ot_state[r] = 1;
-        ot_cv.notify_all();
-        ot_cv.wait(lock, [&] {
-          if (failed.load()) return true;
-          for (uint32_t q = 0; q < r; q++) if (ot_state[q] == 0) return false;
-          return true;
-        });
-        if (failed.load()) { lock.unlock(); ybgpu_job_destroy(job); return; }
-        for (uint32_t q = 0; q < r; q++) doff += ot_dlen[q];
-        ot_meta[r].resize(ml);
-        meta_dst = reinterpret_cast<uint8_t*>(&ot_meta[r][0]);
-      }
-      if (dl) {
-        if (!one) {
-          // 4 KB aligned slices of the caller's arenas, handed out in completion order
-          doff = data_used.fetch_add((dl + 4095) & ~4095ull);
-          moff = meta_used.fetch_add((ml + 4095) & ~4095ull);
-          if (moff + ml > meta_arena_cap) { job_fail(YBGPU_INVALID_ARGUMENT, "output arena too small"); return; }
-          meta_dst = meta_arena + moff;
+      in_slot.Drop();
+      t_added = ms_now();
+      if (added) {
+        s = ybgpu_job_run(job, shutting_down);
+        if (s != YBGPU_OK) { job_fail(s, "run", true); if (failed_or_cut()) return; continue; }
+        if (verify_outputs) {
+          // paranoid_file_checks: the range's table is re-read on its own stream while it is still in device memory; a bad
+          // range fails the compaction before a byte of it reaches the caller's arena
+          ybgpu_output_check chk;
+          s = ybgpu_job_verify_output(job, &chk);
+          if (s != YBGPU_OK) { job_fail(s, "verify_output", true); if (failed_or_cut()) return; continue; }
         }
-        if (doff + dl > data_arena_cap) { job_fail(YBGPU_INVALID_ARGUMENT, "output arena too small"); return; }
-        out_slot.Take(&d2h_gate);
-        t_d2h = ms_now();
-        s = ybgpu_job_fetch_output(job, data_arena + doff, dl, meta_dst, ml);
-        out_slot.Drop();
-        if (s != YBGPU_OK) { job_fail(s, "fetch_output"); return; }
-        out.data_offset = doff; out.data_len = dl; out.meta_offset = moff; out.meta_len = ml;
-        uint64_t sl = 0, ll = 0;
-        uint8_t sk[4096], lk[4096];
-        s = ybgpu_job_output_boundaries(job, sk, &sl, lk, &ll);
-        if (s != YBGPU_OK) { job_fail(s, "output_boundaries"); return; }
-        out.smallest_key_len = static_cast<uint32_t>(std::min<uint64_t>(sl, sizeof(out.smallest_key)));
-        out.largest_key_len = static_cast<uint32_t>(std::min<uint64_t>(ll, sizeof(out.largest_key)));
-        memcpy(out.smallest_key, sk, out.smallest_key_len);
-        memcpy(out.largest_key, lk, out.largest_key_len);
+        if (held && todo.empty()) {
+          // the range has run: from here on it holds no more than what it measured
+          ybgpu_job_stats st;
+          ybgpu_job_get_stats(job, &st);
+          const uint64_t peak = std::min(held, st.device_bytes_peak);
+          unreserve(held - peak);
+          held = peak;
+        }
+        t_ran = ms_now();
+        uint64_t dl = 0, ml = 0;
+        s = ybgpu_job_output_sizes(job, &dl, &ml);
+        if (s != YBGPU_OK) { job_fail(s, "output_sizes"); return; }
+        t_sized = ms_now();
+        uint64_t doff = 0, moff = 0;
+        uint8_t* meta_dst = nullptr;
+        std::string piece_meta;
+        if (one) {
+          // this range's bytes follow those of every earlier range: wait until they all know their sizes (and publish this
+          // range's once its last piece is sized)
+          std::unique_lock<std::mutex> lock(ot_mu);
+          if (todo.empty()) { ot_dlen[r] = r_data + dl; ot_state[r] = 1; ot_cv.notify_all(); }
+          ot_cv.wait(lock, [&] {
+            if (failed.load()) return true;
+            for (uint32_t q = 0; q < r; q++) if (ot_state[q] == 0) return false;
+            return true;
+          });
+          if (failed.load()) { lock.unlock(); destroy(); return; }
+          for (uint32_t q = 0; q < r; q++) doff += ot_dlen[q];
+          doff += r_data;
+          r_data += dl;
+          piece_meta.resize(ml);
+          meta_dst = reinterpret_cast<uint8_t*>(&piece_meta[0]);
+        }
+        if (dl) {
+          if (!one) {
+            // 4 KB aligned slices of the caller's arenas, handed out in completion order
+            doff = data_used.fetch_add((dl + 4095) & ~4095ull);
+            moff = meta_used.fetch_add((ml + 4095) & ~4095ull);
+            if (moff + ml > meta_arena_cap) { job_fail(YBGPU_INVALID_ARGUMENT, "output arena too small"); return; }
+            meta_dst = meta_arena + moff;
+          }
+          if (doff + dl > data_arena_cap) { job_fail(YBGPU_INVALID_ARGUMENT, "output arena too small"); return; }
+          out_slot.Take(&d2h_gate);
+          t_d2h = ms_now();
+          s = ybgpu_job_fetch_output(job, data_arena + doff, dl, meta_dst, ml);
+          out_slot.Drop();
+          if (s != YBGPU_OK) { job_fail(s, "fetch_output"); return; }
+          out.data_offset = doff; out.data_len = dl; out.meta_offset = moff; out.meta_len = ml;
+          uint64_t sl = 0, ll = 0;
+          uint8_t sk[4096], lk[4096];
+          s = ybgpu_job_output_boundaries(job, sk, &sl, lk, &ll);
+          if (s != YBGPU_OK) { job_fail(s, "output_boundaries"); return; }
+          out.smallest_key_len = static_cast<uint32_t>(std::min<uint64_t>(sl, sizeof(out.smallest_key)));
+          out.largest_key_len = static_cast<uint32_t>(std::min<uint64_t>(ll, sizeof(out.largest_key)));
+          memcpy(out.smallest_key, sk, out.smallest_key_len);
+          memcpy(out.largest_key, lk, out.largest_key_len);
+        }
+        t_fetched = ms_now();
+        ybgpu_job_get_stats(job, &out.stats);
+        if (one) ot_meta[r].push_back(std::move(piece_meta));
+      } else if (one) {
+        std::lock_guard<std::mutex> lock(ot_mu);
+        if (todo.empty()) { ot_dlen[r] = r_data; ot_state[r] = 1; ot_cv.notify_all(); }
+        ot_meta[r].emplace_back();
       }
-      t_fetched = ms_now();
-      ybgpu_job_get_stats(job, &out.stats);
+      destroy();
+      subs[r].push_back(out);
+      const double t_destroyed = ms_now();
+      if (trace)
+        fprintf(stderr, "[ybgpu sub] range %2u.%zu: begin %7.1f  inputs in %7.1f  run done %7.1f  meta built %7.1f  d2h start %7.1f  output fetched %7.1f  destroyed %7.1f  (gpu %.1f ms, %.2f GB in)\n",
+                r, subs[r].size() - 1, t_begin, t_added, t_ran, t_sized, t_d2h, t_fetched, t_destroyed, out.stats.gpu_seconds * 1e3, out.stats.h2d_bytes / 1e9);
     }
-    ybgpu_job_destroy(job);
-    const double t_destroyed = ms_now();
+    if (held) { unreserve(held); held = 0; }
     if (one) {
       std::unique_lock<std::mutex> lock(ot_mu);
       ot_state[r] = 2;
       ot_cv.notify_all();
       ot_advance(lock);
     }
-    if (trace)
-      fprintf(stderr, "[ybgpu sub] range %2u: begin %7.1f  inputs in %7.1f  run done %7.1f  meta built %7.1f  d2h start %7.1f  output fetched %7.1f  destroyed %7.1f  assembled %7.1f  (gpu %.1f ms, %.2f GB in)\n",
-              r, t_begin, t_added, t_ran, t_sized, t_d2h, t_fetched, t_destroyed, ms_now(), out.stats.gpu_seconds * 1e3, out.stats.h2d_bytes / 1e9);
   };
 
   auto worker = [&](bool pool_thread) {
@@ -625,13 +769,25 @@ ybgpu_status CompactFilesCore(const ybgpu_job_options* options, const ybgpu_inpu
       if (!e.empty()) return fail(YBGPU_INVALID_ARGUMENT, "one-table assembly: " + e);
     }
   }
+  uint32_t n_out = 0;
+  for (uint32_t r = 0; r < n_ranges; r++) n_out += static_cast<uint32_t>(subs[r].size());
+  if (!one) {
+    if (n_out > output_slots) return fail(YBGPU_INVALID_ARGUMENT, "the budget needed " + std::to_string(n_out) + " ranges, outputs has " +
+                                                                      std::to_string(output_slots) + " slots");
+    uint32_t i = 0;
+    for (uint32_t r = 0; r < n_ranges; r++)
+      for (const ybgpu_sub_output& o : subs[r]) outputs[i++] = o;
+  }
+  *num_outputs = n_out;
   if (total) {
     memset(total, 0, sizeof(*total));
     bool first_output = true;
-    for (uint32_t r = 0; r < n_ranges; r++) {
-      AddStats(total, outputs[r].stats, first_output);
-      if (outputs[r].stats.num_output_records) first_output = false;
-    }
+    for (uint32_t r = 0; r < n_ranges; r++)
+      for (const ybgpu_sub_output& o : subs[r]) {
+        AddStats(total, o.stats, first_output);
+        if (o.stats.num_output_records) first_output = false;
+      }
+    total->device_bytes_peak = mem_group.peak;
   }
   return YBGPU_OK;
 }
@@ -656,8 +812,7 @@ static ybgpu_status CompactFilesOneTable(const ybgpu_job_options* options, const
                                            ybgpu_job_stats* total, char* err, uint64_t err_cap, bool verify_outputs) {
   if (!result || !data_out || !meta_out) { if (err && err_cap) snprintf(err, err_cap, "null argument"); return YBGPU_INVALID_ARGUMENT; }
   memset(result, 0, sizeof(*result));
-  if (max_subcompactions == 0) max_subcompactions = 1;
-  std::vector<ybgpu_sub_output> outs(max_subcompactions);
+  std::vector<ybgpu_sub_output> outs(1);                 // unused: one-table mode keeps the range outputs to itself
   uint32_t n = 0;
   OneTable one;
   ybgpu_job_stats tot;
